@@ -37,6 +37,7 @@ extern "C" {
 #define GB_ITEM_QUEUE_FULL    1   /* best-first frontier exceeded the per-warp workspace    */
 #define GB_ITEM_OUT_FULL      2   /* more extensions / path nodes / mismatches than capacity*/
 #define GB_ITEM_DP_REFUSED    3   /* tail DP refused (cells > max_dozeu_cells), softclipped */
+#define GB_ITEM_NO_BAND       4   /* banded global DP: no global alignment fits inside the band */
 
 /* ------------------------------------------------------------------------------------
  * Flat ("GBZ-flat") index: what GBZ + .min + distance payload become in HBM.
@@ -555,6 +556,27 @@ int gb_sw_batch(gb_device* dev, uint32_t n,
                 const uint8_t* query, const uint64_t* query_off, uint32_t map_cap, uint32_t edit_cap,
                 int32_t* score, gb_mapping* maps, uint32_t* edits, uint32_t* n_maps, uint32_t* n_edits,
                 uint8_t* status);
+
+/* ------------------------------------------------------------------------------------
+ * B3: Aligner::align_global_banded(alignment, graph, band_padding, permissive_banding) — global
+ * alignment from a source to a sink inside vg's per-node diagonal band, regular scoring
+ *                    aligner.cpp:699-761, banded_global_aligner.cpp:251-742, :1961-2266
+ * (the DP fallback for chain middles, minimizer_mapper_from_chains.cpp:2532-3332).
+ * Problems are posed like gb_sw_batch (nodes in topological order + predecessor CSR; sources are the
+ * nodes without predecessors, sinks the nodes without successors in the problem), with
+ * band_padding[i] >= 0 and permissive[i] != 0 for vg's permissive banding.  Queries up to 1024 bases.
+ * Scoring: gb_set_scores without the full-length bonus; a pair with a non-ACGT base scores 0.
+ * Outputs per problem: score, mappings (node = index into the problem's node list, every offset 0),
+ * edits, counts, status: GB_ITEM_NO_BAND when no global alignment fits the band (nothing written),
+ * GB_ITEM_OUT_FULL when the path exceeds map_cap / edit_cap.  An empty query is a deletion of the
+ * shortest source-to-sink path.  Rules and tie-breaking: oracle/banded_global.cpp.
+ * ---------------------------------------------------------------------------------- */
+int gb_banded_global_batch(gb_device* dev, uint32_t n,
+                           const uint32_t* node, const uint64_t* node_off, const uint32_t* pred, const uint64_t* pred_off,
+                           const uint8_t* query, const uint64_t* query_off, const int32_t* band_padding, const uint8_t* permissive,
+                           uint32_t map_cap, uint32_t edit_cap,
+                           int32_t* score, gb_mapping* maps, uint32_t* edits, uint32_t* n_maps, uint32_t* n_edits,
+                           uint8_t* status);
 
 /* ------------------------------------------------------------------------------------
  * B3: Aligner::align_xdrop(alignment, graph, order, mems, reverse_complemented = false, max_gap)

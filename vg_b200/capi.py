@@ -18,6 +18,7 @@ LIB_PATH = ROOT / "vg_b200" / "libgiraffe_b200.so"
 GB_OK = 0
 GB_ERR_ARG, GB_ERR_CUDA, GB_ERR_NO_DEVICE, GB_ERR_CAPACITY, GB_ERR_FORMAT = -1, -2, -3, -4, -5
 GB_ITEM_OK, GB_ITEM_QUEUE_FULL, GB_ITEM_OUT_FULL, GB_ITEM_DP_REFUSED = 0, 1, 2, 3
+GB_ITEM_NO_BAND = 4
 GB_EXT_LEFT_FULL, GB_EXT_RIGHT_FULL = 1, 2
 GB_ALN_MAPPED, GB_ALN_SECONDARY, GB_ALN_PAIRED, GB_ALN_RESCUED, GB_ALN_ABSENT = 1, 2, 4, 8, 16
 GB_MAX_MULTIMAPS = 8
@@ -177,6 +178,8 @@ def load_library() -> C.CDLL:
     lib.gb_xdrop_pinned_batch.restype = C.c_int
     lib.gb_sw_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp]
     lib.gb_sw_batch.restype = C.c_int
+    lib.gb_banded_global_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp]
+    lib.gb_banded_global_batch.restype = C.c_int
     lib.gb_xdrop_dag_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp]
     lib.gb_xdrop_dag_batch.restype = C.c_int
     lib.gb_wfa_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -643,6 +646,46 @@ class Device:
                     ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
                 path.append([int(m["node"]), int(m["offset"]), ed])
             out.append((int(score[i]), path))
+        return out
+
+    def banded_global_batch(self, problems, map_cap=512, edit_cap=2048):
+        """gb_banded_global_batch.  problems: list of (nodes, preds, query bytes, band_padding, permissive)
+        posed like sw_batch.  Returns list of (status, score, path) with path as in sw_batch (empty
+        unless status is GB_ITEM_OK)."""
+        lib = load_library()
+        n = len(problems)
+        node_off = np.zeros(n + 1, dtype=np.uint64)
+        node_off[1:] = np.cumsum([len(p[0]) for p in problems])
+        query_off = np.zeros(n + 1, dtype=np.uint64)
+        query_off[1:] = np.cumsum([len(p[2]) for p in problems])
+        nodes = np.concatenate([np.asarray(p[0], dtype=np.uint32) for p in problems])
+        pred = np.asarray([x for p in problems for ps in p[1] for x in ps] + [0], dtype=np.uint32)
+        pred_off = np.zeros(len(nodes) + 1, dtype=np.uint64)
+        pred_off[1:] = np.cumsum([len(ps) for p in problems for ps in p[1]])
+        q = np.frombuffer(b"".join(bytes(p[2]) for p in problems) + b"\0", dtype=np.uint8).copy()
+        pad = np.asarray([p[3] for p in problems], dtype=np.int32)
+        permissive = np.asarray([1 if p[4] else 0 for p in problems], dtype=np.uint8)
+        score = np.zeros(n, dtype=np.int32)
+        maps = np.zeros(n * map_cap, dtype=mapping_dt)
+        edits = np.zeros(n * edit_cap, dtype=np.uint32)
+        nm = np.zeros(n, dtype=np.uint32); ne = np.zeros(n, dtype=np.uint32)
+        status = np.zeros(n, dtype=np.uint8)
+        rc = lib.gb_banded_global_batch(self._h, n, ptr(nodes), ptr(node_off), ptr(pred), ptr(pred_off), ptr(q), ptr(query_off),
+                                        ptr(pad), ptr(permissive), map_cap, edit_cap, ptr(score), ptr(maps), ptr(edits), ptr(nm),
+                                        ptr(ne), ptr(status))
+        if rc != GB_OK:
+            raise GbError(rc, "gb_banded_global_batch")
+        out = []
+        for i in range(n):
+            path, e = [], i * edit_cap
+            for k in range(int(nm[i])):
+                m = maps[i * map_cap + k]
+                ed = []
+                for _ in range(int(m["n_edits"])):
+                    w = int(edits[e]); e += 1
+                    ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
+                path.append([int(m["node"]), int(m["offset"]), ed])
+            out.append((int(status[i]), int(score[i]), path))
         return out
 
     def xdrop_dag_batch(self, problems, map_cap=512, edit_cap=2048):

@@ -110,15 +110,8 @@ def oracle_banded(index, node, preds, read, pad, permissive, scores=SCORES):
                                   capi.ptr(q), len(read), pad, int(permissive), C.byref(score), capi.ptr(maps), 1024, C.byref(nm),
                                   capi.ptr(edits), 8192, C.byref(ne), C.byref(cells))
     assert rc in (0, 1)
-    path, e = [], 0
-    for i in range(nm.value):
-        ed = []
-        for _ in range(int(maps[i]["n_edits"])):
-            w = int(edits[e]); e += 1
-            ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
-        path.append([int(maps[i]["node"]), int(maps[i]["offset"]), ed])
     status = capi.GB_ITEM_NO_BAND if rc == 1 else capi.GB_ITEM_OK
-    return status, score.value, path
+    return status, score.value, capi.decode_path(maps, edits, nm.value)
 
 
 def path_score(path, seqs, node_of, read, sc):

@@ -12,17 +12,6 @@ from vg_b200 import capi
 GOLD = H.load_golden("sw_local.json")
 
 
-def decode_path(maps, edits, nm):
-    path, e = [], 0
-    for i in range(nm):
-        ed = []
-        for _ in range(int(maps[i]["n_edits"])):
-            w = int(edits[e]); e += 1
-            ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
-        path.append([int(maps[i]["node"]), int(maps[i]["offset"]), ed])
-    return path
-
-
 def oracle_sw(index, problem, read, scores):
     lib = H.oracle_lib()
     lib.oracle_sw_local.restype = C.c_int
@@ -40,7 +29,7 @@ def oracle_sw(index, problem, read, scores):
                              capi.ptr(q), len(read), C.byref(score), capi.ptr(maps), 1024, C.byref(nm), capi.ptr(edits), 4096,
                              C.byref(ne), C.byref(cells))
     assert rc == 0
-    return score.value, decode_path(maps, edits, nm.value), cells.value
+    return score.value, capi.decode_path(maps, edits, nm.value), cells.value
 
 
 def case_index(case):

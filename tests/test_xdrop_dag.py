@@ -51,7 +51,7 @@ def oracle_xdrop_dag(index, nodes, preds, read, scores, seed, max_gap):
                               capi.ptr(q), len(read), su, so, sq, max_gap, C.byref(score), capi.ptr(maps), 1024, C.byref(nm),
                               capi.ptr(edits), 4096, C.byref(ne), C.byref(cells))
     assert rc == 0
-    return score.value, TS.decode_path(maps, edits, nm.value)
+    return score.value, capi.decode_path(maps, edits, nm.value)
 
 
 @pytest.mark.parametrize("seed,qlen,err,gap", [(1, 40, 0.03, 20), (2, 150, 0.05, 60), (3, 250, 0.08, 40), (4, 97, 0.15, 54), (5, 64, 0.3, 30)])

@@ -28,14 +28,7 @@ def oracle_xdrop(index, parents, nodes, root_trim, read, scores, max_gap):
                                  capi.ptr(q), len(read), max_gap, C.byref(score), capi.ptr(maps), 256, C.byref(nm),
                                  capi.ptr(edits), 1024, C.byref(ne))
     assert rc == 0
-    path, e = [], 0
-    for i in range(nm.value):
-        ed = []
-        for _ in range(int(maps[i]["n_edits"])):
-            w = int(edits[e]); e += 1
-            ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
-        path.append([int(maps[i]["node"]), int(maps[i]["offset"]), ed])
-    return score.value, path
+    return score.value, capi.decode_path(maps, edits, nm.value)
 
 
 def case_index(case):

@@ -241,6 +241,41 @@ def ptr(a: np.ndarray) -> C.c_void_p:
     return C.c_void_p(a.ctypes.data)
 
 
+def decode_path(maps, edits, n_maps, node_offset=0):
+    """The first n_maps mappings of maps and their edit words, which start at edits[0], as
+    [[node + node_offset, offset, [[op, length, base], ...]], ...] (base only on substitutions)."""
+    path, e = [], 0
+    for k in range(int(n_maps)):
+        m = maps[k]
+        ed = []
+        for _ in range(int(m["n_edits"])):
+            w = int(edits[e]); e += 1
+            ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
+        path.append([int(m["node"]) + node_offset, int(m["offset"]), ed])
+    return path
+
+
+def _pack_dags(problems):
+    """DAG problems (nodes, preds, query bytes, ...) as the seams' CSR arrays: node, node_off, pred, pred_off, query, query_off."""
+    n = len(problems)
+    node_off = np.zeros(n + 1, dtype=np.uint64)
+    node_off[1:] = np.cumsum([len(p[0]) for p in problems])
+    query_off = np.zeros(n + 1, dtype=np.uint64)
+    query_off[1:] = np.cumsum([len(p[2]) for p in problems])
+    nodes = np.concatenate([np.asarray(p[0], dtype=np.uint32) for p in problems])
+    pred = np.asarray([x for p in problems for ps in p[1] for x in ps] + [0], dtype=np.uint32)
+    pred_off = np.zeros(len(nodes) + 1, dtype=np.uint64)
+    pred_off[1:] = np.cumsum([len(ps) for p in problems for ps in p[1]])
+    q = np.frombuffer(b"".join(bytes(p[2]) for p in problems) + b"\0", dtype=np.uint8).copy()
+    return nodes, node_off, pred, pred_off, q, query_off
+
+
+def _seam_outputs(n, map_cap, edit_cap):
+    """The output arrays of a batched alignment seam: score, maps, edits, n_maps, n_edits, status."""
+    return (np.zeros(n, dtype=np.int32), np.zeros(n * map_cap, dtype=mapping_dt), np.zeros(n * edit_cap, dtype=np.uint32),
+            np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint8))
+
+
 class GbError(RuntimeError):
     def __init__(self, code: int, what: str):
         msg = load_library().gb_last_error()
@@ -585,28 +620,15 @@ class Device:
         trim = np.array([p[2] for p in problems], dtype=np.uint32)
         q = np.frombuffer(b"".join(bytes(p[3]) for p in problems) + b"\0", dtype=np.uint8).copy()
         gap = np.array([p[4] for p in problems], dtype=np.uint32)
-        score = np.zeros(n, dtype=np.int32)
-        maps = np.zeros(n * map_cap, dtype=mapping_dt)
-        edits = np.zeros(n * edit_cap, dtype=np.uint32)
-        nm = np.zeros(n, dtype=np.uint32); ne = np.zeros(n, dtype=np.uint32)
-        status = np.zeros(n, dtype=np.uint8)
+        score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
         rc = lib.gb_xdrop_pinned_batch(self._h, n, ptr(par), ptr(nodes), ptr(tree_off), ptr(trim), ptr(q), ptr(query_off),
-                                       ptr(gap), map_cap, edit_cap, ptr(score), ptr(maps), ptr(edits), ptr(nm), ptr(ne),
-                                       ptr(status))
+                                       ptr(gap), map_cap, edit_cap, *map(ptr, outs))
         if rc != GB_OK:
             raise GbError(rc, "gb_xdrop_pinned_batch")
         out = []
         for i in range(n):
             assert status[i] == GB_ITEM_OK, f"problem {i}: status {status[i]}"
-            path, e = [], i * edit_cap
-            for k in range(int(nm[i])):
-                m = maps[i * map_cap + k]
-                ed = []
-                for _ in range(int(m["n_edits"])):
-                    w = int(edits[e]); e += 1
-                    ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
-                path.append([int(m["node"]) + 1, int(m["offset"]), ed])
-            out.append((int(score[i]), path))
+            out.append((int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i], node_offset=1)))
         return out
 
     def sw_batch(self, problems, map_cap=512, edit_cap=2048):
@@ -615,37 +637,15 @@ class Device:
         Returns list of (score, [[problem_index, offset, [[op, len, base], ...]], ...])."""
         lib = load_library()
         n = len(problems)
-        node_off = np.zeros(n + 1, dtype=np.uint64)
-        node_off[1:] = np.cumsum([len(p[0]) for p in problems])
-        query_off = np.zeros(n + 1, dtype=np.uint64)
-        query_off[1:] = np.cumsum([len(p[2]) for p in problems])
-        nodes = np.concatenate([np.asarray(p[0], dtype=np.uint32) for p in problems])
-        flat_pred = [x for p in problems for ps in p[1] for x in ps]
-        pred = np.asarray(flat_pred + [0], dtype=np.uint32)
-        pred_off = np.zeros(len(nodes) + 1, dtype=np.uint64)
-        pred_off[1:] = np.cumsum([len(ps) for p in problems for ps in p[1]])
-        q = np.frombuffer(b"".join(bytes(p[2]) for p in problems) + b"\0", dtype=np.uint8).copy()
-        score = np.zeros(n, dtype=np.int32)
-        maps = np.zeros(n * map_cap, dtype=mapping_dt)
-        edits = np.zeros(n * edit_cap, dtype=np.uint32)
-        nm = np.zeros(n, dtype=np.uint32); ne = np.zeros(n, dtype=np.uint32)
-        status = np.zeros(n, dtype=np.uint8)
-        rc = lib.gb_sw_batch(self._h, n, ptr(nodes), ptr(node_off), ptr(pred), ptr(pred_off), ptr(q), ptr(query_off),
-                             map_cap, edit_cap, ptr(score), ptr(maps), ptr(edits), ptr(nm), ptr(ne), ptr(status))
+        dags = _pack_dags(problems)
+        score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
+        rc = lib.gb_sw_batch(self._h, n, *map(ptr, dags), map_cap, edit_cap, *map(ptr, outs))
         if rc != GB_OK:
             raise GbError(rc, "gb_sw_batch")
         out = []
         for i in range(n):
             assert status[i] == GB_ITEM_OK, f"problem {i}: status {status[i]}"
-            path, e = [], i * edit_cap
-            for k in range(int(nm[i])):
-                m = maps[i * map_cap + k]
-                ed = []
-                for _ in range(int(m["n_edits"])):
-                    w = int(edits[e]); e += 1
-                    ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
-                path.append([int(m["node"]), int(m["offset"]), ed])
-            out.append((int(score[i]), path))
+            out.append((int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i])))
         return out
 
     def banded_global_batch(self, problems, map_cap=512, edit_cap=2048):
@@ -654,77 +654,33 @@ class Device:
         unless status is GB_ITEM_OK)."""
         lib = load_library()
         n = len(problems)
-        node_off = np.zeros(n + 1, dtype=np.uint64)
-        node_off[1:] = np.cumsum([len(p[0]) for p in problems])
-        query_off = np.zeros(n + 1, dtype=np.uint64)
-        query_off[1:] = np.cumsum([len(p[2]) for p in problems])
-        nodes = np.concatenate([np.asarray(p[0], dtype=np.uint32) for p in problems])
-        pred = np.asarray([x for p in problems for ps in p[1] for x in ps] + [0], dtype=np.uint32)
-        pred_off = np.zeros(len(nodes) + 1, dtype=np.uint64)
-        pred_off[1:] = np.cumsum([len(ps) for p in problems for ps in p[1]])
-        q = np.frombuffer(b"".join(bytes(p[2]) for p in problems) + b"\0", dtype=np.uint8).copy()
         pad = np.asarray([p[3] for p in problems], dtype=np.int32)
         permissive = np.asarray([1 if p[4] else 0 for p in problems], dtype=np.uint8)
-        score = np.zeros(n, dtype=np.int32)
-        maps = np.zeros(n * map_cap, dtype=mapping_dt)
-        edits = np.zeros(n * edit_cap, dtype=np.uint32)
-        nm = np.zeros(n, dtype=np.uint32); ne = np.zeros(n, dtype=np.uint32)
-        status = np.zeros(n, dtype=np.uint8)
-        rc = lib.gb_banded_global_batch(self._h, n, ptr(nodes), ptr(node_off), ptr(pred), ptr(pred_off), ptr(q), ptr(query_off),
-                                        ptr(pad), ptr(permissive), map_cap, edit_cap, ptr(score), ptr(maps), ptr(edits), ptr(nm),
-                                        ptr(ne), ptr(status))
+        dags = _pack_dags(problems)
+        score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
+        rc = lib.gb_banded_global_batch(self._h, n, *map(ptr, dags), ptr(pad), ptr(permissive), map_cap, edit_cap,
+                                        *map(ptr, outs))
         if rc != GB_OK:
             raise GbError(rc, "gb_banded_global_batch")
-        out = []
-        for i in range(n):
-            path, e = [], i * edit_cap
-            for k in range(int(nm[i])):
-                m = maps[i * map_cap + k]
-                ed = []
-                for _ in range(int(m["n_edits"])):
-                    w = int(edits[e]); e += 1
-                    ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
-                path.append([int(m["node"]), int(m["offset"]), ed])
-            out.append((int(status[i]), int(score[i]), path))
-        return out
+        return [(int(status[i]), int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i])) for i in range(n)]
 
     def xdrop_dag_batch(self, problems, map_cap=512, edit_cap=2048):
         """gb_xdrop_dag_batch.  problems: list of (nodes, preds, query bytes, seed or None, max_gap) with
         seed = (node index, node offset, query offset).  Returns list of (score, path) like sw_batch."""
         lib = load_library()
         n = len(problems)
-        node_off = np.zeros(n + 1, dtype=np.uint64)
-        node_off[1:] = np.cumsum([len(p[0]) for p in problems])
-        query_off = np.zeros(n + 1, dtype=np.uint64)
-        query_off[1:] = np.cumsum([len(p[2]) for p in problems])
-        nodes = np.concatenate([np.asarray(p[0], dtype=np.uint32) for p in problems])
-        pred = np.asarray([x for p in problems for ps in p[1] for x in ps] + [0], dtype=np.uint32)
-        pred_off = np.zeros(len(nodes) + 1, dtype=np.uint64)
-        pred_off[1:] = np.cumsum([len(ps) for p in problems for ps in p[1]])
-        q = np.frombuffer(b"".join(bytes(p[2]) for p in problems) + b"\0", dtype=np.uint8).copy()
         seed = np.array([(0xFFFFFFFF, 0, 0) if p[3] is None else p[3] for p in problems], dtype=np.uint32).reshape(-1)
         gap = np.array([p[4] for p in problems], dtype=np.uint32)
-        score = np.zeros(n, dtype=np.int32)
-        maps = np.zeros(n * map_cap, dtype=mapping_dt)
-        edits = np.zeros(n * edit_cap, dtype=np.uint32)
-        nm = np.zeros(n, dtype=np.uint32); ne = np.zeros(n, dtype=np.uint32)
-        status = np.zeros(n, dtype=np.uint8)
-        rc = lib.gb_xdrop_dag_batch(self._h, n, ptr(nodes), ptr(node_off), ptr(pred), ptr(pred_off), ptr(q), ptr(query_off),
-                                    ptr(seed), ptr(gap), map_cap, edit_cap, ptr(score), ptr(maps), ptr(edits), ptr(nm), ptr(ne), ptr(status))
+        dags = _pack_dags(problems)
+        score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
+        rc = lib.gb_xdrop_dag_batch(self._h, n, *map(ptr, dags), ptr(seed), ptr(gap), map_cap, edit_cap,
+                                    *map(ptr, outs))
         if rc != GB_OK:
             raise GbError(rc, "gb_xdrop_dag_batch")
         out = []
         for i in range(n):
             assert status[i] == GB_ITEM_OK, f"problem {i}: status {status[i]}"
-            path, e = [], i * edit_cap
-            for k in range(int(nm[i])):
-                m = maps[i * map_cap + k]
-                ed = []
-                for _ in range(int(m["n_edits"])):
-                    w = int(edits[e]); e += 1
-                    ed.append(["MSID"[w & 3], w >> 4, "ACGT"[(w >> 2) & 3] if (w & 3) == 1 else ""])
-                path.append([int(m["node"]), int(m["offset"]), ed])
-            out.append((int(score[i]), path))
+            out.append((int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i])))
         return out
 
     def chain_candidates_batch(self, problems, limit=2 ** 64 - 1, cap=None):

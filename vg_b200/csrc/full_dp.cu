@@ -13,26 +13,18 @@
 #include "giraffe_b200.h"
 #include "device_state.cuh"
 #include "dag_dp.cuh"
-
-#include <algorithm>
-#include <vector>
+#include "seam_batch.cuh"
 
 namespace gb {
 
 constexpr int SW_WARPS = 4;
 
 struct SwBatch {
-    const uint32_t* node; const uint64_t* node_off;         // problem p: nodes node_off[p] .. node_off[p+1] (topological order)
-    const uint32_t* pred; const uint64_t* pred_off;         // CSR over all nodes (global node index): predecessor indices within the problem
-    const uint8_t* query; const uint64_t* query_off;
-    uint32_t n; uint32_t Lc;
-    int32_t* score; gb_mapping* maps; uint32_t* edits; uint32_t* n_maps; uint32_t* n_edits; uint8_t* status;
-    uint32_t map_cap, edit_cap;
-    // per-problem workspace offsets (host prefix sums)
-    int32_t* lastH; int32_t* lastE; uint8_t* argH; uint8_t* argE; const uint64_t* col_off;    // node-granular: (global node index) * W_p via col_off[p] + u * W
-    uint8_t* tb; const uint64_t* tb_off;                    // byte offset of problem p's traceback matrix
+    DagDev dag;
+    SeamOut out;
+    // per-node workspaces, offset by the problem's first global node: node-granular columns at col_off[p] + u * (m + 1)
+    int32_t* lastH; int32_t* lastE; uint8_t* argH; uint8_t* argE;
     uint32_t* col_start; uint32_t* seq_off; uint32_t* seq_len;   // per global node: first traceback column, sequence
-    uint32_t* steps; const uint64_t* step_off;
     uint32_t* work_counter;
 };
 
@@ -40,32 +32,26 @@ __global__ void __launch_bounds__(SW_WARPS * 32)
 sw_kernel(DevIndex ix, DevScores sc, SwBatch b) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t W = b.Lc + 1;
-    const size_t per_warp = (((size_t)b.Lc + 15) & ~(size_t)15) + (size_t)W * 4 * 4 + 64;
-    uint8_t* base = smem + (size_t)warp * per_warp;
-    uint8_t* q = base;
-    int32_t* cols = reinterpret_cast<int32_t*>(base + (((size_t)b.Lc + 15) & ~(size_t)15));
-    DpSmem dps; dps.Hp = cols; dps.Ep = cols + W; dps.Hc = cols + 2 * W; dps.Ec = cols + 3 * W;
+    uint8_t* q;
+    const DpSmem dps = dp_smem_carve(smem, warp, b.dag.Lc, q);
     while (true) {
         uint32_t p = 0;
         if (lane == 0) p = atomicAdd(b.work_counter, 1u);
         p = __shfl_sync(FULL, p, 0);
-        if (p >= b.n) break;
+        if (p >= b.dag.n) break;
         uint32_t status = GB_ITEM_OK; int32_t score = 0;
-        PathBuf out; out.maps = b.maps + (size_t)p * b.map_cap; out.edits = b.edits + (size_t)p * b.edit_cap;
-        out.map_cap = b.map_cap; out.edit_cap = b.edit_cap; pb_reset(out);
+        PathBuf out = b.out.path(p);
         {
-            const uint64_t n0 = b.node_off[p];
             DagView v;
-            v.N = (uint32_t)(b.node_off[p + 1] - n0); v.node = b.node + n0;
-            v.pred = b.pred; v.pred_off = b.pred_off + n0; v.succ = nullptr; v.succ_off = nullptr;
+            const uint64_t n0 = b.dag.view(p, v), c0 = b.dag.col_off[p];
+            v.succ = nullptr; v.succ_off = nullptr;
             v.col_start = b.col_start + n0; v.seq_off = b.seq_off + n0; v.seq_len = b.seq_len + n0; v.nstate = nullptr;
-            v.lastH = b.lastH + b.col_off[p]; v.lastE = b.lastE + b.col_off[p]; v.argH = b.argH + b.col_off[p]; v.argE = b.argE + b.col_off[p];
-            v.tb = b.tb + b.tb_off[p]; v.steps = b.steps + b.step_off[p];
-            const uint64_t q0 = b.query_off[p];
-            sw_align(ix, sc, v, b.query + q0, (uint32_t)(b.query_off[p + 1] - q0), q, dps, score, out, status);
+            v.lastH = b.lastH + c0; v.lastE = b.lastE + c0; v.argH = b.argH + c0; v.argE = b.argE + c0;
+            uint32_t m;
+            const uint8_t* read = b.dag.read(p, m);
+            sw_align(ix, sc, v, read, m, q, dps, score, out, status);
         }
-        if (lane == 0) { b.score[p] = status == GB_ITEM_OK ? score : 0; b.n_maps[p] = out.n_maps; b.n_edits[p] = out.n_edits; b.status[p] = (uint8_t)status; }
+        b.out.store(p, status == GB_ITEM_OK ? score : 0, out.n_maps, out.n_edits, status);
         __syncwarp();
     }
 }
@@ -82,81 +68,19 @@ extern "C" int gb_sw_batch(gb_device* d, uint32_t n,
         !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
     if (n == 0) return GB_OK;
     GB_CUDA(cudaSetDevice(d->device));
-    const uint64_t total_nodes = node_off[n], total_pred = pred_off[total_nodes], total_q = query_off[n];
-    // validate the DAG shape (predecessors precede, known nodes, at most 255 predecessors) and size the workspaces
-    uint32_t max_q = 0;
-    std::vector<uint64_t> col_off(n + 1, 0), tb_off(n + 1, 0), step_off(n + 1, 0);
-    for (uint32_t p = 0; p < n; p++) {
-        const uint32_t m = (uint32_t)(query_off[p + 1] - query_off[p]);
-        max_q = std::max(max_q, m);
-        uint64_t bases = 0;
-        const uint64_t N = node_off[p + 1] - node_off[p];
-        for (uint64_t u = 0; u < N; u++) {
-            const uint32_t v = node[node_off[p] + u];
-            if (v < 2 || v >= d->ix.n_nodes) { g_last_error = "gb_sw_batch: unknown node"; return GB_ERR_ARG; }
-            const uint64_t g = node_off[p] + u;
-            if (pred_off[g + 1] - pred_off[g] > 255) { g_last_error = "gb_sw_batch: more than 255 predecessors"; return GB_ERR_ARG; }
-            for (uint64_t e = pred_off[g]; e < pred_off[g + 1]; e++)
-                if (pred[e] >= u) { g_last_error = "gb_sw_batch: nodes are not in topological order"; return GB_ERR_ARG; }
-        }
-        // node lengths live on the device; bound the traceback by the host copy of the index sizes instead:
-        // every node is at most 1023 bases (position encoding), the exact sum is taken below from d->h_node_len
-        for (uint64_t u = 0; u < N; u++) bases += d->h_node_len[node[node_off[p] + u]];
-        col_off[p + 1] = col_off[p] + N * (uint64_t)(m + 1);
-        tb_off[p + 1] = tb_off[p] + bases * (uint64_t)(m + 1);
-        step_off[p + 1] = step_off[p] + bases + m + 2;
-    }
-    const uint32_t Lc = std::max<uint32_t>(32u, (max_q + 15u) & ~15u);
-    if (Lc > 1024) { g_last_error = "query too long"; return GB_ERR_ARG; }
-    if (tb_off[n] > (uint64_t)8 << 30) { g_last_error = "gb_sw_batch: batch needs more than 8 GiB of traceback"; return GB_ERR_CAPACITY; }
-    DevBuf<uint32_t> d_node, d_pred, d_edits, d_nm, d_ne, d_counter, d_colstart, d_seqoff, d_seqlen, d_steps;
-    DevBuf<uint64_t> d_noff, d_poff, d_qoff, d_coloff, d_tboff, d_stepoff;
-    DevBuf<int32_t> d_score, d_lastH, d_lastE; DevBuf<uint8_t> d_q, d_status, d_argH, d_argE, d_tb; DevBuf<gb_mapping> d_maps;
-    int rc;
-    if ((rc = d_node.upload(node, total_nodes ? total_nodes : 1, d->stream, total_nodes))) return rc;
-    if ((rc = d_pred.upload(pred, total_pred ? total_pred : 1, d->stream, total_pred))) return rc;
-    if ((rc = d_noff.upload(node_off, n + 1, d->stream))) return rc;
-    if ((rc = d_poff.upload(pred_off, total_nodes + 1, d->stream))) return rc;
-    if ((rc = d_q.upload(query, total_q ? total_q : 1, d->stream, total_q))) return rc;
-    if ((rc = d_qoff.upload(query_off, n + 1, d->stream))) return rc;
-    if ((rc = d_coloff.upload(col_off.data(), n + 1, d->stream))) return rc;
-    if ((rc = d_tboff.upload(tb_off.data(), n + 1, d->stream))) return rc;
-    if ((rc = d_stepoff.upload(step_off.data(), n + 1, d->stream))) return rc;
-    if ((rc = d_score.reserve(n)) || (rc = d_nm.reserve(n)) || (rc = d_ne.reserve(n)) || (rc = d_status.reserve(n))) return rc;
-    if ((rc = d_maps.reserve((size_t)n * map_cap)) || (rc = d_edits.reserve((size_t)n * edit_cap))) return rc;
-    if ((rc = d_lastH.reserve(col_off[n] + 1)) || (rc = d_lastE.reserve(col_off[n] + 1))) return rc;
-    if ((rc = d_argH.reserve(col_off[n] + 1)) || (rc = d_argE.reserve(col_off[n] + 1))) return rc;
-    if ((rc = d_tb.reserve(tb_off[n] + 1)) || (rc = d_steps.reserve(step_off[n] + 1))) return rc;
-    if ((rc = d_colstart.reserve(total_nodes + 1)) || (rc = d_seqoff.reserve(total_nodes + 1)) || (rc = d_seqlen.reserve(total_nodes + 1))) return rc;
-    if ((rc = d_counter.reserve(4))) return rc;
-    GB_CUDA(cudaMemsetAsync(d_counter.ptr, 0, 16, d->stream));
-    const uint32_t W = Lc + 1;
-    const size_t per_warp = (((size_t)Lc + 15) & ~(size_t)15) + (size_t)W * 4 * 4 + 64;
-    const size_t smem = per_warp * SW_WARPS;
-    if (smem > 48 * 1024) GB_CUDA(cudaFuncSetAttribute(sw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int bps = 0;
-    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, sw_kernel, SW_WARPS * 32, smem));
-    if (bps < 1) bps = 1;
-    const uint32_t grid = std::max<uint32_t>(1u, std::min<uint32_t>((uint32_t)d->n_sms * bps, (n + SW_WARPS - 1) / SW_WARPS));
+    DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
+    SeamOutBufs out;
+    DevBuf<int32_t> d_lastH, d_lastE; DevBuf<uint8_t> d_argH, d_argE; DevBuf<uint32_t> d_colstart, d_seqoff, d_seqlen;
     SwBatch b;
-    b.node = d_node.ptr; b.node_off = d_noff.ptr; b.pred = d_pred.ptr; b.pred_off = d_poff.ptr; b.query = d_q.ptr; b.query_off = d_qoff.ptr;
-    b.n = n; b.Lc = Lc; b.score = d_score.ptr; b.maps = d_maps.ptr; b.edits = d_edits.ptr; b.n_maps = d_nm.ptr; b.n_edits = d_ne.ptr;
-    b.status = d_status.ptr; b.map_cap = map_cap; b.edit_cap = edit_cap;
-    b.lastH = d_lastH.ptr; b.lastE = d_lastE.ptr; b.argH = d_argH.ptr; b.argE = d_argE.ptr; b.col_off = d_coloff.ptr;
-    b.tb = d_tb.ptr; b.tb_off = d_tboff.ptr; b.col_start = d_colstart.ptr; b.seq_off = d_seqoff.ptr; b.seq_len = d_seqlen.ptr;
-    b.steps = d_steps.ptr; b.step_off = d_stepoff.ptr; b.work_counter = d_counter.ptr;
-    GB_CUDA(cudaEventRecord(d->ev0, d->stream));
-    sw_kernel<<<grid, SW_WARPS * 32, smem, d->stream>>>(d->ix, d->sc, b);
-    d->launches++;
-    GB_CUDA(cudaGetLastError());
-    GB_CUDA(cudaEventRecord(d->ev1, d->stream));
-    GB_CUDA(cudaMemcpyAsync(score, d_score.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(n_maps, d_nm.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(n_edits, d_ne.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(status, d_status.ptr, n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(maps, d_maps.ptr, sizeof(gb_mapping) * (size_t)n * map_cap, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(edits, d_edits.ptr, 4 * (size_t)n * edit_cap, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaStreamSynchronize(d->stream));
-    GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
-    return GB_OK;
+    int rc;
+    if ((rc = dag.validate(d, "gb_sw_batch")) || (rc = dag.check_limits("gb_sw_batch")) || (rc = dag.upload(d->stream, b.dag))) return rc;
+    const uint64_t cols = dag.col_off[n] + 1, nodes = dag.total_nodes + 1;
+    if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
+    if ((rc = d_lastH.reserve(cols)) || (rc = d_lastE.reserve(cols)) || (rc = d_argH.reserve(cols)) || (rc = d_argE.reserve(cols))) return rc;
+    if ((rc = d_colstart.reserve(nodes)) || (rc = d_seqoff.reserve(nodes)) || (rc = d_seqlen.reserve(nodes))) return rc;
+    b.out = out.view;
+    b.lastH = d_lastH.ptr; b.lastE = d_lastE.ptr; b.argH = d_argH.ptr; b.argE = d_argE.ptr;
+    b.col_start = d_colstart.ptr; b.seq_off = d_seqoff.ptr; b.seq_len = d_seqlen.ptr;
+    if ((rc = launch_warp_per_problem(d, sw_kernel, b, SW_WARPS, dp_smem_per_warp(dag.Lc) * SW_WARPS))) return rc;
+    return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
 }

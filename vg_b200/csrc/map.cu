@@ -9,6 +9,7 @@
 #include "align.cuh"
 #include "extend.cuh"
 #include "dag_dp.cuh"
+#include "seam_batch.cuh"
 
 #include <algorithm>
 #include <cfloat>
@@ -848,8 +849,7 @@ struct XdropBatch {
     const int32_t* tree_parent; const uint32_t* tree_node; const uint64_t* tree_off; const uint32_t* root_trim;
     const uint8_t* query; const uint64_t* query_off; const uint32_t* max_gap;
     uint32_t n; uint32_t Lc;
-    int32_t* score; gb_mapping* maps; uint32_t* edits; uint32_t* n_maps; uint32_t* n_edits; uint8_t* status;
-    uint32_t map_cap, edit_cap;
+    SeamOut out;
     uint8_t* ws_base; size_t ws_stride; uint32_t tb_cells;
     uint32_t* work_counter;
     const uint8_t* skip;             // [n] 1: the problem runs on xdrop_tile_kernel instead
@@ -862,14 +862,15 @@ __global__ void unpack_tile_results_kernel(XdropBatch b, const TileResult* resul
     if (p >= b.n || !b.skip[p]) return;
     const TileResult tr = results[p];
     uint32_t status = tr.status == GB_TILE_ST_OK ? (uint32_t)GB_ITEM_OK : (uint32_t)GB_ITEM_OUT_FULL;
-    if (status == GB_ITEM_OK && (tr.n_maps > b.map_cap || tr.n_edits > b.edit_cap)) status = GB_ITEM_OUT_FULL;
+    if (status == GB_ITEM_OK && (tr.n_maps > b.out.map_cap || tr.n_edits > b.out.edit_cap)) status = GB_ITEM_OUT_FULL;
     if (status == GB_ITEM_OK) {
         const gb_mapping* gm = reinterpret_cast<const gb_mapping*>(path_pool + tr.path_off);
         const uint32_t* ge = path_pool + tr.path_off + 2 * tr.n_maps;
-        for (uint32_t i = lane; i < tr.n_maps; i += 32) b.maps[(size_t)p * b.map_cap + i] = gm[i];
-        for (uint32_t i = lane; i < tr.n_edits; i += 32) b.edits[(size_t)p * b.edit_cap + i] = ge[i];
+        for (uint32_t i = lane; i < tr.n_maps; i += 32) b.out.maps[(size_t)p * b.out.map_cap + i] = gm[i];
+        for (uint32_t i = lane; i < tr.n_edits; i += 32) b.out.edits[(size_t)p * b.out.edit_cap + i] = ge[i];
     }
-    if (lane == 0) { b.score[p] = status == GB_ITEM_OK ? tr.score : 0; b.n_maps[p] = status == GB_ITEM_OK ? tr.n_maps : 0; b.n_edits[p] = status == GB_ITEM_OK ? tr.n_edits : 0; b.status[p] = (uint8_t)status; }
+    const bool ok = status == GB_ITEM_OK;
+    b.out.store(p, ok ? tr.score : 0, ok ? tr.n_maps : 0, ok ? tr.n_edits : 0, status);
 }
 
 __global__ void __launch_bounds__(ALIGN_WARPS * 32, 4)
@@ -877,12 +878,8 @@ xdrop_kernel(DevIndex ix, DevScores sc, XdropBatch b) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t gwarp = blockIdx.x * ALIGN_WARPS + warp;
-    const uint32_t W = b.Lc + 1;
-    const size_t per_warp = (((size_t)b.Lc + 15) & ~(size_t)15) + (size_t)W * 4 * 4 + 64;
-    uint8_t* base = smem + (size_t)warp * per_warp;
-    uint8_t* q = base;
-    int32_t* cols = reinterpret_cast<int32_t*>(base + (((size_t)b.Lc + 15) & ~(size_t)15));
-    DpSmem dps; dps.Hp = cols; dps.Ep = cols + W; dps.Hc = cols + 2 * W; dps.Ec = cols + 3 * W;
+    uint8_t* q;
+    const DpSmem dps = dp_smem_carve(smem, warp, b.Lc, q);
     const TailWs ws = carve_tail_ws(b.ws_base + (size_t)gwarp * b.ws_stride, b.Lc, b.tb_cells);
     while (true) {
         uint32_t p = 0;
@@ -893,8 +890,7 @@ xdrop_kernel(DevIndex ix, DevScores sc, XdropBatch b) {
         const uint64_t t_begin = b.tree_off[p]; const uint32_t nt = (uint32_t)(b.tree_off[p + 1] - t_begin);
         const uint64_t q_begin = b.query_off[p]; const uint32_t m = (uint32_t)(b.query_off[p + 1] - q_begin);
         uint32_t status = GB_ITEM_OK; int32_t score = 0;
-        PathBuf out; out.maps = b.maps + (size_t)p * b.map_cap; out.edits = b.edits + (size_t)p * b.edit_cap;
-        out.map_cap = b.map_cap; out.edit_cap = b.edit_cap; pb_reset(out);
+        PathBuf out = b.out.path(p);
         if (nt == 0 || nt > TAIL_T_CAP || m > b.Lc) status = GB_ITEM_OUT_FULL;
         else {
             for (uint32_t i = lane; i < m; i += 32) q[i] = dp_query_base(b.query[q_begin + i]);
@@ -915,7 +911,7 @@ xdrop_kernel(DevIndex ix, DevScores sc, XdropBatch b) {
             score = xdrop_tree(ix, sc, ws, dps, 0, nt, q, m, max(b.max_gap[p], 1u), out, ovf);
             if (ovf || out.overflow) status = GB_ITEM_OUT_FULL;
         }
-        if (lane == 0) { b.score[p] = score; b.n_maps[p] = out.n_maps; b.n_edits[p] = out.n_edits; b.status[p] = (uint8_t)status; }
+        b.out.store(p, score, out.n_maps, out.n_edits, status);
         __syncwarp();
     }
 }
@@ -932,13 +928,12 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
         !edits || !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
     if (n == 0) return GB_OK;
     GB_CUDA(cudaSetDevice(d->device));
-    uint32_t max_q = 0;
+    uint32_t max_q = 0, Lc;
     for (uint32_t i = 0; i < n; i++) max_q = std::max<uint32_t>(max_q, (uint32_t)(query_off[i + 1] - query_off[i]));
-    const uint32_t Lc = std::max<uint32_t>(32u, (max_q + 15u) & ~15u);
-    if (Lc > 1024) { g_last_error = "query too long"; return GB_ERR_ARG; }
-    DevBuf<int32_t> d_par, d_score; DevBuf<uint32_t> d_node, d_trim, d_gap, d_edits, d_nm, d_ne, d_counter; DevBuf<uint64_t> d_toff, d_qoff;
-    DevBuf<uint8_t> d_q, d_status, d_ws; DevBuf<gb_mapping> d_maps;
     int rc;
+    if ((rc = query_columns(max_q, Lc))) return rc;
+    DevBuf<int32_t> d_par; DevBuf<uint32_t> d_node, d_trim, d_gap, d_counter; DevBuf<uint64_t> d_toff, d_qoff;
+    DevBuf<uint8_t> d_q, d_ws; SeamOutBufs out;
     const uint64_t nt = tree_off[n], nq = query_off[n];
     if ((rc = d_par.upload(tree_parent, nt ? nt : 1, d->stream, nt))) return rc;
     if ((rc = d_node.upload(tree_node, nt ? nt : 1, d->stream, nt))) return rc;
@@ -947,14 +942,10 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
     if ((rc = d_gap.upload(max_gap, n, d->stream))) return rc;
     if ((rc = d_q.upload(query, nq ? nq : 1, d->stream, nq))) return rc;
     if ((rc = d_qoff.upload(query_off, n + 1, d->stream))) return rc;
-    if ((rc = d_score.reserve(n))) return rc; if ((rc = d_nm.reserve(n))) return rc; if ((rc = d_ne.reserve(n))) return rc;
-    if ((rc = d_status.reserve(n))) return rc;
-    if ((rc = d_maps.reserve((size_t)n * map_cap))) return rc; if ((rc = d_edits.reserve((size_t)n * edit_cap))) return rc;
+    if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
     if ((rc = d_counter.reserve(4))) return rc;
     GB_CUDA(cudaMemsetAsync(d_counter.ptr, 0, 16, d->stream));
-    const uint32_t W = Lc + 1;
-    const size_t per_warp = (((size_t)Lc + 15) & ~(size_t)15) + (size_t)W * 4 * 4 + 64;
-    const size_t smem = per_warp * ALIGN_WARPS;
+    const size_t smem = dp_smem_per_warp(Lc) * ALIGN_WARPS;
     if (smem > 48 * 1024) GB_CUDA(cudaFuncSetAttribute(xdrop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     uint32_t grid = std::min<uint32_t>((uint32_t)d->n_sms * 2, (n + ALIGN_WARPS - 1) / ALIGN_WARPS);
     const uint32_t tb_cells = 2 * 1024 * 1024;
@@ -962,9 +953,8 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
     if ((rc = d_ws.reserve(ws_stride * grid * ALIGN_WARPS))) return rc;
     XdropBatch b;
     b.tree_parent = d_par.ptr; b.tree_node = d_node.ptr; b.tree_off = d_toff.ptr; b.root_trim = d_trim.ptr;
-    b.query = d_q.ptr; b.query_off = d_qoff.ptr; b.max_gap = d_gap.ptr; b.n = n; b.Lc = Lc;
-    b.score = d_score.ptr; b.maps = d_maps.ptr; b.edits = d_edits.ptr; b.n_maps = d_nm.ptr; b.n_edits = d_ne.ptr; b.status = d_status.ptr;
-    b.map_cap = map_cap; b.edit_cap = edit_cap; b.ws_base = d_ws.ptr; b.ws_stride = ws_stride; b.tb_cells = tb_cells;
+    b.query = d_q.ptr; b.query_off = d_qoff.ptr; b.max_gap = d_gap.ptr; b.n = n; b.Lc = Lc; b.out = out.view;
+    b.ws_base = d_ws.ptr; b.ws_stride = ws_stride; b.tb_cells = tb_cells;
     b.work_counter = d_counter.ptr;
     // ---- problems the int16 tile kernel can hold run there (the production path of the tails); the rest on the int32 sweep ----
     std::vector<uint8_t> elig(n, 0); std::vector<uint32_t> toff(n, 0);
@@ -1017,13 +1007,5 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
     }
     d->last_tile_problems = n_elig;
     GB_CUDA(cudaEventRecord(d->ev1, d->stream));
-    GB_CUDA(cudaMemcpyAsync(score, d_score.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(n_maps, d_nm.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(n_edits, d_ne.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(status, d_status.ptr, n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(maps, d_maps.ptr, sizeof(gb_mapping) * (size_t)n * map_cap, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(edits, d_edits.ptr, 4 * (size_t)n * edit_cap, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaStreamSynchronize(d->stream));
-    GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
-    return GB_OK;
+    return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
 }

@@ -184,6 +184,21 @@ __device__ inline uint32_t build_tail_forest(const DevIndex& ix, const TailWs& w
 // -----------------------------------------------------------------------------------------
 struct DpSmem { int32_t *Hp, *Ep, *Hc, *Ec; };
 
+// Dynamic shared memory per warp of the one-warp DP kernels (sw_kernel, xdrop_dag_kernel, xdrop_kernel):
+// the staged query (Lc bytes, rounded up to 16), then the four DP columns of Lc + 1 cells, then 64 spare bytes.
+__host__ __device__ inline size_t dp_smem_per_warp(uint32_t Lc) {
+    return (((size_t)Lc + 15) & ~(size_t)15) + ((size_t)Lc + 1) * 4 * 4 + 64;
+}
+// warp `warp`'s query buffer (q) and DP columns within that layout
+__device__ inline DpSmem dp_smem_carve(uint8_t* smem, int warp, uint32_t Lc, uint8_t*& q) {
+    uint8_t* base = smem + (size_t)warp * dp_smem_per_warp(Lc);
+    q = base;
+    int32_t* cols = reinterpret_cast<int32_t*>(base + (((size_t)Lc + 15) & ~(size_t)15));
+    const uint32_t W = Lc + 1;
+    DpSmem dps; dps.Hp = cols; dps.Ep = cols + W; dps.Hc = cols + 2 * W; dps.Ec = cols + 3 * W;
+    return dps;
+}
+
 __device__ inline int32_t xdrop_tree(const DevIndex& ix, const DevScores& sc, const TailWs& ws, DpSmem dps,
                                      uint32_t t0, uint32_t t1, const uint8_t* q, uint32_t m, uint32_t max_gap,
                                      PathBuf& out, bool& overflow) {

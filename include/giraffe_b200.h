@@ -529,6 +529,17 @@ int gb_plan_stats(gb_device* dev, uint64_t* out4);
  * Outputs per problem: score, mappings (node = tree index, offsets in trimmed coordinates),
  * edits, counts.  Right-pinned problems are posed, as the reference does
  * (minimizer_mapper.cpp:5663-5665), on the reverse-complemented query and reverse tree.
+ * A problem's status is GB_ITEM_OUT_FULL when its path needs more than map_cap mappings or
+ * edit_cap edits, more than 4096 traceback steps (query bases plus deleted bases), or, on the
+ * int32 sweep, more than 2048 tree nodes or 2^21 traceback cells.  A problem the int16 tile
+ * kernel can hold never exceeds the sweep's node and cell limits, and a tile that outgrows its
+ * own path buffers is recomputed on the sweep, so which kernel ran it does not change the answer.
+ * Returns GB_ERR_ARG, before anything is uploaded, when map_cap or edit_cap is 0, a query is
+ * longer than 1024 bases, or a tree is malformed: no nodes, a node id below 2 or not in the
+ * index, a first node whose parent is not negative, a later node whose parent is negative (a
+ * second root), not below its own index or not on the path from the root to the node before
+ * it (not DFS visit order), a root_trim not below the root's length, or a node 512 or more
+ * levels below the root.
  * ---------------------------------------------------------------------------------- */
 int gb_xdrop_pinned_batch(gb_device* dev, uint32_t n,
                           const int32_t* tree_parent, const uint32_t* tree_node, const uint64_t* tree_off,

@@ -28,6 +28,9 @@ def oracle_lib_configure(lib):
     lib.oracle_bd_state.restype = C.c_int
     lib.oracle_follow_paths.argtypes = [C.POINTER(capi.FlatIndex), vp, C.c_int, vp, C.c_int]
     lib.oracle_follow_paths.restype = C.c_int
+    lib.oracle_xdrop_pinned.argtypes = [C.POINTER(capi.FlatIndex), C.POINTER(capi.Scores), vp, vp, u32, u32, vp, u32, u32, vp,
+                                        vp, u32, vp, vp, u32, vp]
+    lib.oracle_xdrop_pinned.restype = C.c_int
     return lib
 
 

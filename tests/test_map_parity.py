@@ -148,6 +148,74 @@ def test_map_parity_with_the_tile_kernels_switched_off(monkeypatch):
     assert want[4]["tail_dps"] > 1000 and plan["cells"] == 0 and plan["tails"] == 0
 
 
+def _reads_with_one_indel(g, n, lengths, dist, seed):
+    """n reads of lengths[0] .. lengths[1] bp copied from the haplotypes, each with one 1-3 bp insertion or deletion
+    dist[0] .. dist[1] bases from its left or right end, half of them reverse complemented."""
+    rng = np.random.default_rng(seed)
+    reads = []
+    for _ in range(n):
+        hs = g.hap_seq[int(rng.integers(0, len(g.hap_seq)))]
+        L = int(rng.integers(lengths[0], lengths[1] + 1))
+        s = int(rng.integers(0, len(hs) - L - 8))
+        seq = hs[s: s + L + 8]
+        d = int(rng.integers(dist[0], dist[1] + 1))
+        at = d if rng.random() < 0.5 else L - d
+        k = int(rng.integers(1, 4))
+        if rng.random() < 0.5:
+            seq = np.concatenate([seq[:at], synth.BASES[rng.integers(0, 4, size=k)], seq[at:]])
+        else:
+            seq = np.concatenate([seq[:at], seq[at + k:]])
+        seq = seq[:L]
+        reads.append(bytes(synth.revcomp_bytes(seq) if rng.random() < 0.5 else seq))
+    return reads, [bytes([30] * len(r)) for r in reads]
+
+
+def _run_tiles_on_and_off(monkeypatch, index, reads, quals, params):
+    """The records with the tile kernels and with GIRAFFE_B200_TILES=0 both equal the oracle's; plan stats of the
+    tiled run."""
+    want = H.oracle_map(index, reads, quals, params, threads=8)
+    plan = None
+    for tiles in ("1", "0"):
+        monkeypatch.setenv("GIRAFFE_B200_TILES", tiles)
+        dev = capi.Device(index)
+        got = H.gpu_map(dev, reads, quals, params)
+        if tiles == "1":
+            plan = dev.plan_stats()
+        dev.close()
+        bad = H.compare_alignments(got, want, len(reads))
+        assert not bad, f"tiles={tiles}: {len(bad)} of {len(reads)} reads differ; first: read {bad[0][0]}\n got={bad[0][1]}\nwant={bad[0][2]}"
+    return plan, want
+
+
+@pytest.mark.gpu
+def test_map_parity_with_tails_longer_than_a_tile_path(monkeypatch):
+    """2-bp nodes and 300-400 bp reads with an indel 100-150 bases from one end: the far tail's path has more mappings
+    than a tile's result holds (96).  With the read's caps raised to 512 mappings / 1024 edits such a tail is aligned
+    in place, and the records are the same with and without the tile kernels.  Chunks of 128 reads keep the
+    extensions of every read within the large-stride extension pool (n_reads / 128 + 256 work items per chunk): nearly
+    every read here outgrows the regular 384-node extension stride."""
+    monkeypatch.setenv("GIRAFFE_B200_MAP_CHUNK", "128")
+    g = synth.make_variant_graph(length=60000, n_snp=100, n_ins=12, n_del=12, n_haps=8, seed=6, max_node=2)
+    reads, quals = _reads_with_one_indel(g, 600, (300, 400), (100, 150), seed=61)
+    p = capi.default_map_params()
+    p.mapping_cap_per_read = 512
+    p.edit_cap_per_read = 1024
+    plan, want = _run_tiles_on_and_off(monkeypatch, g.build_index(), reads, quals, p)
+    assert want[4]["tail_dps"] > 500 and plan["cells"] > 0
+    assert (want[0]["n_mappings"] > 96).sum() > 300
+
+
+@pytest.mark.gpu
+def test_map_parity_long_reads_with_long_tails(monkeypatch):
+    """400-512 bp reads with an indel 40-80 bases from either end on 32-bp nodes: the extension on the short side has a
+    tail of at least 320 bases (the 12- and 16-row tile classes when tail_plan plans it; left tails through the
+    reverse-complement translation, GB_TILE_LEFT)."""
+    g = synth.make_variant_graph(length=200000, n_snp=320, n_ins=40, n_del=40, n_haps=8, seed=2)
+    reads, quals = _reads_with_one_indel(g, 1000, (400, 512), (40, 80), seed=62)
+    plan, want = _run_tiles_on_and_off(monkeypatch, g.build_index(), reads, quals, None)
+    assert want[4]["tail_dps"] > 500 and plan["tails"] > 500 and plan["cells"] > 0
+
+
 @pytest.mark.gpu
 def test_map_parity_with_scaled_scores_on_tiles_and_sweeps():
     """Scoring parameters x20: tile_scores_fit_int16 accepts the short tails and rejects the long ones, so one batch mixes

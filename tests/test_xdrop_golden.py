@@ -13,10 +13,6 @@ GOLD = H.load_golden("xdrop_pinned.json")
 
 def oracle_xdrop(index, parents, nodes, root_trim, read, scores, max_gap):
     lib = H.oracle_lib()
-    lib.oracle_xdrop_pinned.restype = C.c_int
-    lib.oracle_xdrop_pinned.argtypes = [C.POINTER(capi.FlatIndex), C.POINTER(capi.Scores), C.c_void_p, C.c_void_p,
-                                        C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p,
-                                        C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
     par = np.asarray(parents, dtype=np.int32)
     nd = np.asarray(nodes, dtype=np.uint32)
     q = np.frombuffer(read.encode() + b"\0", dtype=np.uint8).copy()

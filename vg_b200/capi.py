@@ -606,9 +606,11 @@ class Device:
             raise GbError(rc, "gb_extend_batch")
         return ext_count, status, ext, path_pool, mism_pool
 
-    def xdrop_pinned_batch(self, problems, map_cap=256, edit_cap=1024):
+    def xdrop_pinned_batch(self, problems, map_cap=256, edit_cap=1024, with_status=False):
         """problems: list of (parents, nodes, root_trim, query bytes, max_gap).
-        Returns list of (score, [[tree_index + 1, offset, [[op, len, base], ...]], ...])."""
+        Returns list of (score, [[tree_index + 1, offset, [[op, len, base], ...]], ...]), every status
+        asserted GB_ITEM_OK; with_status=True returns (status, score, path) instead, path empty unless
+        status is GB_ITEM_OK."""
         lib = load_library()
         n = len(problems)
         tree_off = np.zeros(n + 1, dtype=np.uint64)
@@ -625,6 +627,10 @@ class Device:
                                        ptr(gap), map_cap, edit_cap, *map(ptr, outs))
         if rc != GB_OK:
             raise GbError(rc, "gb_xdrop_pinned_batch")
+        if with_status:
+            return [(int(status[i]), int(score[i]),
+                     decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i], node_offset=1) if status[i] == GB_ITEM_OK else [])
+                    for i in range(n)]
         out = []
         for i in range(n):
             assert status[i] == GB_ITEM_OK, f"problem {i}: status {status[i]}"

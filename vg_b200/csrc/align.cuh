@@ -242,10 +242,13 @@ __device__ inline int32_t align_tail(const DevIndex& ix, const MapParamsDev& P, 
 #pragma unroll 1
         for (uint32_t x = 0; x < tl.count; x++) if (tl.pv->entries[tl.base + x].key == tl.key) { pe = tl.pv->entries + tl.base + x; break; }
         // a cancelled tail (the decide pass judged that the reference skips it, :5478-5492) is never asked for; should the
-        // walk here disagree, the tail is simply aligned in place
+        // walk here disagree, the tail is simply aligned in place.  So is a tail with a tile that ran out of the tile's
+        // fixed path capacities (TILE_MAP_CAP / TILE_EDIT_CAP / TILE_STEP_CAP): the in-place sweep writes into the
+        // read's own buffers, whose caps the caller sets.  The check comes before any RNG draw, so the draw order is
+        // the in-place loop's either way.
         if (pe) for (uint32_t t = 0; t < pe->n_trees; t++) {
             const uint32_t ti = pe->first_tile + t;
-            if (tl.pv->tile_off[ti] != TILE_REFUSED && tl.pv->results[ti].status == GB_TILE_ST_CANCELLED) { pe = nullptr; break; }
+            if (tl.pv->tile_off[ti] != TILE_REFUSED && tl.pv->results[ti].status != GB_TILE_ST_OK) { pe = nullptr; break; }
         }
         if (pe) {
             int32_t best_score = 0;
@@ -257,7 +260,6 @@ __device__ inline int32_t align_tail(const DevIndex& ix, const MapParamsDev& P, 
                 const uint32_t ti = pe->first_tile + t;
                 if (tl.pv->tile_off[ti] == TILE_REFUSED) continue;            // subgraph too large for max_dozeu_cells (:5694-5701)
                 const TileResult tr = tl.pv->results[ti];
-                if (tr.status != GB_TILE_ST_OK) { status = GB_ITEM_OUT_FULL; return 0; }
                 bool beats = false;
                 if (tr.score > best_score) beats = true;
                 else if (tr.score == best_score) beats = (rng_next(rng) % 2) != 0;

@@ -852,17 +852,23 @@ struct XdropBatch {
     SeamOut out;
     uint8_t* ws_base; size_t ws_stride; uint32_t tb_cells;
     uint32_t* work_counter;
-    const uint8_t* skip;             // [n] 1: the problem runs on xdrop_tile_kernel instead
+    uint8_t* skip;                   // [n] 1: the problem ran on xdrop_tile_kernel instead
 };
 
-// results of the tile kernel -> the seam's output arrays
+// results of the tile kernel -> the seam's output arrays.  A tile that outgrew the tile's own path capacities
+// (TILE_MAP_CAP / TILE_EDIT_CAP / TILE_STEP_CAP) gives its problem back to xdrop_kernel, which aligns it within the
+// caller's map_cap / edit_cap: the seam's answer does not depend on which kernel a problem was routed to.
 __global__ void unpack_tile_results_kernel(XdropBatch b, const TileResult* results, const uint32_t* path_pool) {
     const uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (p >= b.n || !b.skip[p]) return;
     const TileResult tr = results[p];
-    uint32_t status = tr.status == GB_TILE_ST_OK ? (uint32_t)GB_ITEM_OK : (uint32_t)GB_ITEM_OUT_FULL;
-    if (status == GB_ITEM_OK && (tr.n_maps > b.out.map_cap || tr.n_edits > b.out.edit_cap)) status = GB_ITEM_OUT_FULL;
+    if (tr.status != GB_TILE_ST_OK) {
+        if (lane == 0) b.skip[p] = 0;
+        return;
+    }
+    uint32_t status = GB_ITEM_OK;
+    if (tr.n_maps > b.out.map_cap || tr.n_edits > b.out.edit_cap) status = GB_ITEM_OUT_FULL;
     if (status == GB_ITEM_OK) {
         const gb_mapping* gm = reinterpret_cast<const gb_mapping*>(path_pool + tr.path_off);
         const uint32_t* ge = path_pool + tr.path_off + 2 * tr.n_maps;
@@ -927,11 +933,38 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
     if (!d || !tree_parent || !tree_node || !tree_off || !root_trim || !query || !query_off || !max_gap || !score || !maps ||
         !edits || !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
     if (n == 0) return GB_OK;
-    GB_CUDA(cudaSetDevice(d->device));
+    // ---- validation, before anything reaches the device: known nodes; one root, first; the nodes in DFS visit order (both
+    // kernels keep one DP column per tree level, which a node's parent must still own); the root trim leaves a base; fewer
+    // than TAIL_D_CAP levels ----
+    std::vector<uint64_t> prob_bases(n, 0); std::vector<uint32_t> prob_depth(n, 0), lineage;
     uint32_t max_q = 0, Lc;
-    for (uint32_t i = 0; i < n; i++) max_q = std::max<uint32_t>(max_q, (uint32_t)(query_off[i + 1] - query_off[i]));
+    auto fail = [](const char* what) { g_last_error = std::string("gb_xdrop_pinned_batch: ") + what; return GB_ERR_ARG; };
+    for (uint32_t i = 0; i < n; i++) {
+        max_q = std::max<uint32_t>(max_q, (uint32_t)(query_off[i + 1] - query_off[i]));
+        const uint64_t t0 = tree_off[i]; const uint32_t ntree = (uint32_t)(tree_off[i + 1] - t0);
+        if (ntree == 0) return fail("empty tree");
+        lineage.clear();                      // root .. previous node
+        for (uint32_t x = 0; x < ntree; x++) {
+            const uint32_t v = tree_node[t0 + x]; const int32_t par = tree_parent[t0 + x];
+            if (v < 2 || v >= d->ix.n_nodes || d->h_node_len[v] == 0) return fail("unknown node");
+            if (x == 0 && par >= 0) return fail("the first tree node is not a root");
+            if (x > 0 && par < 0) return fail("more than one root");
+            if (par >= (int32_t)x) return fail("a parent does not precede its child");
+            while (par >= 0 && !lineage.empty() && lineage.back() != (uint32_t)par) lineage.pop_back();
+            if (par >= 0 && lineage.empty()) return fail("tree nodes are not in DFS visit order");
+            lineage.push_back(x);
+            const uint32_t len = d->h_node_len[v];
+            if (par < 0) {
+                if (root_trim[i] >= len) return fail("root_trim leaves no base of the root");
+                prob_bases[i] += len - root_trim[i];
+            } else prob_bases[i] += len;
+            if (lineage.size() > TAIL_D_CAP) return fail("tree deeper than 511 levels");
+            prob_depth[i] = std::max<uint32_t>(prob_depth[i], (uint32_t)lineage.size() - 1);
+        }
+    }
     int rc;
     if ((rc = query_columns(max_q, Lc))) return rc;
+    GB_CUDA(cudaSetDevice(d->device));
     DevBuf<int32_t> d_par; DevBuf<uint32_t> d_node, d_trim, d_gap, d_counter; DevBuf<uint64_t> d_toff, d_qoff;
     DevBuf<uint8_t> d_q, d_ws; SeamOutBufs out;
     const uint64_t nt = tree_off[n], nq = query_off[n];
@@ -961,20 +994,10 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
     uint64_t units = 0; uint32_t n_elig = 0;
     if (d->use_tiles) {
         for (uint32_t i = 0; i < n; i++) {
-            const uint64_t t0 = tree_off[i]; const uint32_t ntree = (uint32_t)(tree_off[i + 1] - t0), m = (uint32_t)(query_off[i + 1] - query_off[i]);
-            if (ntree == 0 || ntree > TILE_MAX_NODES) continue;
-            uint64_t bases = 0; uint32_t max_depth = 0; bool ok = true;
-            std::vector<uint32_t> depth(ntree, 0);
-            for (uint32_t x = 0; x < ntree && ok; x++) {
-                const uint32_t v = tree_node[t0 + x]; const int32_t par = tree_parent[t0 + x];
-                if (v >= d->h_node_len.size() || par >= (int32_t)x) { ok = false; break; }
-                const uint32_t len = d->h_node_len[v];
-                if (par < 0) { if (root_trim[i] >= len) { ok = false; break; } bases += len - root_trim[i]; }
-                else { bases += len; depth[x] = depth[par] + 1; max_depth = std::max(max_depth, depth[x]); }
-            }
-            if (!ok || tree_parent[t0] >= 0) continue;
-            if (!tile_eligible(d->sc, m, std::max(max_gap[i], 1u), ntree, (uint32_t)std::min<uint64_t>(bases, 0xffffffffu), max_depth)) continue;
-            elig[i] = 1; toff[i] = (uint32_t)units; units += tile_bytes(ntree, (uint32_t)bases, m) / 16; n_elig++;
+            const uint32_t ntree = (uint32_t)(tree_off[i + 1] - tree_off[i]), m = (uint32_t)(query_off[i + 1] - query_off[i]);
+            const uint32_t bases = (uint32_t)std::min<uint64_t>(prob_bases[i], 0xffffffffu);
+            if (!tile_eligible(d->sc, m, std::max(max_gap[i], 1u), ntree, bases, prob_depth[i])) continue;
+            elig[i] = 1; toff[i] = (uint32_t)units; units += tile_bytes(ntree, bases, m) / 16; n_elig++;
         }
     }
     DevBuf<uint8_t> d_elig, d_tiles; DevBuf<uint32_t> d_tileoff, d_lists, d_tc, d_paths; DevBuf<TileResult> d_res;
@@ -1000,11 +1023,11 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
         d->launches++;
         GB_CUDA(cudaGetLastError());
     } else b.skip = nullptr;
-    if (n_elig < n) {
-        xdrop_kernel<<<grid, ALIGN_WARPS * 32, smem, d->stream>>>(d->ix, d->sc, b);
-        d->launches++;
-        GB_CUDA(cudaGetLastError());
-    }
+    // the int32 sweep takes the problems not eligible for a tile and those whose tile ended FULL; the latter are known only
+    // on the device, so it runs after the tiles too and skips the problems they finished
+    xdrop_kernel<<<grid, ALIGN_WARPS * 32, smem, d->stream>>>(d->ix, d->sc, b);
+    d->launches++;
+    GB_CUDA(cudaGetLastError());
     d->last_tile_problems = n_elig;
     GB_CUDA(cudaEventRecord(d->ev1, d->stream));
     return out.download(d, n, score, maps, edits, n_maps, n_edits, status);

@@ -21,7 +21,7 @@ constexpr int32_t DP_NEG = INT_MIN / 4;
 constexpr uint32_t TAIL_T_CAP = 2048;     // tree nodes per forest
 constexpr uint32_t TAIL_S_CAP = 2048;     // DFS stack frames
 constexpr uint32_t TAIL_D_CAP = 512;      // tree depth
-constexpr uint32_t TAIL_STEP_CAP = 2048;  // traceback steps
+constexpr uint32_t TAIL_STEP_CAP = 4096;  // traceback steps (TILE_STEP_CAP of xdrop_tile.cuh: a path fits both kernels or neither)
 
 struct TreeNode {
     int32_t parent;        // index in the forest array, -1 for a tree root

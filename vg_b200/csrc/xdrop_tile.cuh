@@ -426,7 +426,10 @@ __device__ __noinline__ int32_t xdrop_tile_dp(const DevScores& sc, const uint8_t
         uint32_t pf_node = 0xffffffffu, pf_col = 0, pf_j = 0, pf_byte = 0;
         while (!ovf) {
             if (at_virtual) {
-                for (; j > 0; j--) step(0, 2u, 0);                   // leading insertion in the virtual column, on the root
+                for (; j > 0; j--) {                                 // leading insertion in the virtual column, on the root
+                    if (n_steps >= TILE_STEP_CAP) TILE_FAIL(6);      // the same step count as the int32 sweep's TAIL_STEP_CAP
+                    step(0, 2u, 0);
+                }
                 break;
             }
             const TileNode tn = nodes[node];

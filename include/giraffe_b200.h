@@ -618,9 +618,21 @@ int gb_xdrop_dag_batch(gb_device* dev, uint32_t n,
  * nodes; the unused end is ignored).  error_model: 12 numbers {per_base, min, max} for mismatches,
  * gaps, gap length, distance (WFAExtender::ErrorModel, gbwt_extender.hpp:340-385), NULL = defaults.
  * Outputs per problem, as the fields of WFAAlignment (gbwt_extender.hpp:233-307): ok (0: no
- * alignment, 1: alignment, -1: workspace capacity exceeded), score, node_offset, seq_offset, length,
- * path (oriented nodes, at most path_cap), edits as (length << 2) | op with op 0 match, 1 mismatch,
- * 2 insertion, 3 deletion (at most edit_cap).
+ * alignment, 1: alignment, -1: see below), score, node_offset, seq_offset, length, path (oriented
+ * nodes, at most path_cap), edits as (length << 2) | op with op 0 match, 1 mismatch, 2 insertion,
+ * 3 deletion (at most edit_cap).
+ * Each problem runs in a fixed workspace.  ok is -1, with score and counts 0, exactly when the
+ * problem needs more than one of: 64 haplotype-trie nodes, 24 576 bytes of trie node sequence,
+ * 2 048 graph nodes over all trie nodes, 3 071 stored wavefront points (over the three matrices
+ * and all trie nodes), 512 distinct possible scores, 32 successors of one trie node; or stores a
+ * point with score 8192 or more, a diagonal outside [-1024, 1024), or a sequence or node offset
+ * above 65 535; or when the returned path (after its unused first and trailing nodes are dropped)
+ * has more than path_cap nodes or its edits more than edit_cap runs.  A trie node grows along a
+ * non-branching haplotype until it holds 1 024 bases, so the trie can hold far more graph nodes
+ * than the returned path.  The kernel first tries a 256-cell point table (191 points) and redoes a
+ * problem that fills it with the whole table; GIRAFFE_B200_WFA_SMALL_TABLE=0, read on every call,
+ * starts with the whole table.  Returns GB_ERR_ARG when path_cap or edit_cap is 0, a mode is above
+ * 2 or a sequence is longer than 60 000 bases; n = 0 returns GB_OK without a launch.
  * ---------------------------------------------------------------------------------- */
 int gb_wfa_batch(gb_device* dev, uint32_t n, const uint8_t* seq, const uint64_t* seq_off, const uint32_t* mode,
                  const uint32_t* pos, const double* error_model, uint32_t path_cap, uint32_t edit_cap,

@@ -72,6 +72,9 @@ struct Tree {
     int32_t mismatch, gap_open, gap_extend, score_bound = 0, max_distance = 0, min_distance = 0;
     struct ScoreProperties { int32_t min_diagonal, max_diagonal; bool reachable_with_gap; };
     std::map<int32_t, ScoreProperties> possible_scores;
+    // what gb_wfa_batch's fixed per-problem workspace would have needed (oracle_wfa_workspace)
+    uint32_t max_successors = 0; int32_t max_point_score = 0, min_point_diagonal = 0, max_point_diagonal = 0;
+    uint32_t max_point_seq_offset = 0, max_point_node_offset = 0;
 
     // WFANode::append_node
     bool append_node(Node& n, const SearchState& next) {
@@ -101,9 +104,8 @@ struct Tree {
         : graph(g), sequence(seq), to_node(to_node_), to_offset(to_offset_), has_to(has_to_),
           mismatch(2 * (sc.match + sc.mismatch)), gap_open(2 * (sc.gap_open - sc.gap_extend)), gap_extend(2 * sc.gap_extend + sc.match) {
         SearchState st; st.node = from_node; st.lo = 0; st.hi = (int64_t)g.record_size(from_node) - 1;
-        Node root = make_node(st, 0);
-        root.wf[MATCHES][{0, 0}] = {0u, from_offset + 1};
-        nodes.push_back(std::move(root));
+        nodes.push_back(make_node(st, 0));
+        update(nodes[0], MATCHES, 0, 0, 0u, from_offset + 1);
         const int32_t max_mismatches = em.mismatches.evaluate(seq.length());
         const int32_t max_gaps = em.gaps.evaluate(seq.length());
         const int32_t max_gap_length = em.gap_length.evaluate(seq.length());
@@ -115,7 +117,12 @@ struct Tree {
     int32_t gap_extend_penalty(uint32_t length) const { return (int32_t)length * gap_extend; }
     int32_t gap_penalty(uint32_t length) const { return gap_open + gap_extend_penalty(length); }
 
-    static void update(Node& n, int type, int32_t score, int32_t diagonal, uint32_t seq_offset, uint32_t node_offset) { n.wf[type][{score, diagonal}] = {seq_offset, node_offset}; }
+    void update(Node& n, int type, int32_t score, int32_t diagonal, uint32_t seq_offset, uint32_t node_offset) {
+        n.wf[type][{score, diagonal}] = {seq_offset, node_offset};
+        max_point_score = std::max(max_point_score, score);
+        min_point_diagonal = std::min(min_point_diagonal, diagonal); max_point_diagonal = std::max(max_point_diagonal, diagonal);
+        max_point_seq_offset = std::max(max_point_seq_offset, seq_offset); max_point_node_offset = std::max(max_point_node_offset, node_offset);
+    }
     void update(int type, int32_t score, int32_t diagonal, const Pos& p) { update(nodes[p.node()], type, score, diagonal, p.seq_offset, p.node_offset); }
 
     std::vector<uint32_t> get_leaves() const { std::vector<uint32_t> l; for (uint32_t i = 0; i < size(); i++) if (nodes[i].is_leaf()) l.push_back(i); return l; }
@@ -145,6 +152,7 @@ struct Tree {
         bool found = false;
         std::vector<SearchState> kids;
         graph.follow_paths(nodes[node].state, [&](const SearchState& child) -> bool { kids.push_back(child); return true; });
+        max_successors = std::max(max_successors, (uint32_t)kids.size());
         for (const SearchState& child : kids) {
             nodes[node].children.push_back(size());
             Node n = make_node(child, node);
@@ -338,9 +346,27 @@ struct Alignment {
 
 static void mask(std::string& s) { for (char& c : s) if (c != 'A' && c != 'C' && c != 'G' && c != 'T') c = 'X'; }
 
+// What one problem needs of gb_wfa_batch's per-problem workspace, measured when the wavefront loop stops (the kernel
+// follows the same trajectory, so these are the maxima it meets).  Order of the fields: oracle_wfa_workspace.
+struct Workspace {
+    uint32_t trie_nodes = 0, seq_bytes = 0, path_entries = 0, points = 0, scores = 0;
+    int32_t max_score = 0, min_diagonal = 0, max_diagonal = 0;
+    uint32_t max_seq_offset = 0, max_node_offset = 0, max_successors = 0;
+};
+static void report(const Tree& t, Workspace& w) {
+    w.trie_nodes = t.size();
+    for (const Node& n : t.nodes) {
+        w.seq_bytes += (uint32_t)n.seq.size(); w.path_entries += (uint32_t)n.path.size();
+        for (int k = 0; k < 3; k++) w.points += (uint32_t)n.wf[k].size();
+    }
+    w.scores = (uint32_t)t.possible_scores.size();
+    w.max_score = t.max_point_score; w.min_diagonal = t.min_point_diagonal; w.max_diagonal = t.max_point_diagonal;
+    w.max_seq_offset = t.max_point_seq_offset; w.max_node_offset = t.max_point_node_offset; w.max_successors = t.max_successors;
+}
+
 // WFAExtender::connect (to_node == 0: no destination)
 Alignment connect(const Graph& g, const gb_scores& sc, const ErrorModel& em, std::string sequence,
-                  uint32_t from_node, uint32_t from_offset, uint32_t to_node, uint32_t to_offset) {
+                  uint32_t from_node, uint32_t from_offset, uint32_t to_node, uint32_t to_offset, Workspace* ws = nullptr) {
     Alignment fail;
     if (!g.has_node(from_node)) return fail;
     mask(sequence);
@@ -356,6 +382,7 @@ Alignment connect(const Graph& g, const gb_scores& sc, const ErrorModel& em, std
         if (score > tree.score_bound) break;
         tree.next(score);
     }
+    if (ws) report(tree, *ws);
     bool full_length = true;
     uint32_t unaligned_tail = (uint32_t)(sequence.length() - tree.candidate_point.seq_offset);
     if (tree.candidate_point.score > tree.score_bound) {
@@ -430,8 +457,9 @@ Alignment connect(const Graph& g, const gb_scores& sc, const ErrorModel& em, std
     return result;
 }
 
-Alignment suffix(const Graph& g, const gb_scores& sc, const ErrorModel& em, const std::string& sequence, uint32_t from_node, uint32_t from_offset) {
-    Alignment r = connect(g, sc, em, sequence, from_node, from_offset, 0, 0);
+Alignment suffix(const Graph& g, const gb_scores& sc, const ErrorModel& em, const std::string& sequence, uint32_t from_node, uint32_t from_offset,
+                 Workspace* ws = nullptr) {
+    Alignment r = connect(g, sc, em, sequence, from_node, from_offset, 0, 0, ws);
     if (!r.edits.empty() && r.length == sequence.length() && (r.edits.back().first == MATCH || r.edits.back().first == MISMATCH)) r.score += sc.full_length_bonus;
     return r;
 }
@@ -442,11 +470,12 @@ static std::string revcomp(const std::string& s) {
     return r;
 }
 
-Alignment prefix(const Graph& g, const gb_scores& sc, const ErrorModel& em, const std::string& sequence, uint32_t to_node, uint32_t to_offset) {
+Alignment prefix(const Graph& g, const gb_scores& sc, const ErrorModel& em, const std::string& sequence, uint32_t to_node, uint32_t to_offset,
+                 Workspace* ws = nullptr) {
     if (!g.has_node(to_node)) return Alignment();
     // reverse_base_pos: the same base on the other strand
     const uint32_t rnode = to_node ^ 1u, roff = g.get_length(to_node) - 1 - to_offset;
-    Alignment r = connect(g, sc, em, revcomp(sequence), rnode, roff, 0, 0);
+    Alignment r = connect(g, sc, em, revcomp(sequence), rnode, roff, 0, 0, ws);
     r.flip(g, sequence.length());
     if (!r.edits.empty() && r.length == sequence.length() && (r.edits.front().first == MATCH || r.edits.front().first == MISMATCH)) r.score += sc.full_length_bonus;
     return r;
@@ -459,26 +488,50 @@ Alignment prefix(const Graph& g, const gb_scores& sc, const ErrorModel& em, cons
 // offset); error_model = 12 numbers {per_base, min, max} x {mismatches, gaps, gap_length, distance}
 // (nullptr: WFAExtender::ErrorModel defaults, gbwt_extender.hpp:372-381).
 // Output: ok flag, score, node_offset, seq_offset, length, path (oriented nodes), edits as (length << 2) | op.
-extern "C" int oracle_wfa(const gb_flat_index* ix, const gb_scores* scores, const double* error_model, int mode,
-                          const uint8_t* seq, uint32_t seq_len, uint32_t from_node, uint32_t from_offset, uint32_t to_node, uint32_t to_offset,
-                          int32_t* ok, int32_t* score, uint32_t* node_offset, uint32_t* seq_offset, uint32_t* length,
-                          uint32_t* path, uint32_t path_cap, uint32_t* n_path, uint32_t* edits, uint32_t edit_cap, uint32_t* n_edits) {
+static oracle::wfa::Alignment run_wfa(const oracle::Graph& g, const gb_scores* scores, const double* error_model, int mode,
+                                      const uint8_t* seq, uint32_t seq_len, uint32_t from_node, uint32_t from_offset, uint32_t to_node, uint32_t to_offset,
+                                      oracle::wfa::Workspace* ws) {
     using namespace oracle::wfa;
-    oracle::Graph g(ix);
     ErrorModel em{{0.03, 1, 6}, {0.05, 1, 10}, {0.1, 1, 20}, {0.1, 10, 200}};
     if (error_model) {
         const double* e = error_model;
         em = ErrorModel{{e[0], (int32_t)e[1], (int32_t)e[2]}, {e[3], (int32_t)e[4], (int32_t)e[5]}, {e[6], (int32_t)e[7], (int32_t)e[8]}, {e[9], (int32_t)e[10], (int32_t)e[11]}};
     }
     const std::string s((const char*)seq, seq_len);
-    Alignment a;
-    if (mode == 0) a = connect(g, *scores, em, s, from_node, from_offset, to_node, to_offset);
-    else if (mode == 1) a = suffix(g, *scores, em, s, from_node, from_offset);
-    else a = prefix(g, *scores, em, s, to_node, to_offset);
+    if (mode == 0) return connect(g, *scores, em, s, from_node, from_offset, to_node, to_offset, ws);
+    if (mode == 1) return suffix(g, *scores, em, s, from_node, from_offset, ws);
+    return prefix(g, *scores, em, s, to_node, to_offset, ws);
+}
+
+// C entry.  mode: 0 connect(from, to), 1 suffix(from), 2 prefix(to).  Positions are (oriented node,
+// offset); error_model = 12 numbers {per_base, min, max} x {mismatches, gaps, gap_length, distance}
+// (nullptr: WFAExtender::ErrorModel defaults, gbwt_extender.hpp:372-381).
+// Output: ok flag, score, node_offset, seq_offset, length, path (oriented nodes), edits as (length << 2) | op.
+extern "C" int oracle_wfa(const gb_flat_index* ix, const gb_scores* scores, const double* error_model, int mode,
+                          const uint8_t* seq, uint32_t seq_len, uint32_t from_node, uint32_t from_offset, uint32_t to_node, uint32_t to_offset,
+                          int32_t* ok, int32_t* score, uint32_t* node_offset, uint32_t* seq_offset, uint32_t* length,
+                          uint32_t* path, uint32_t path_cap, uint32_t* n_path, uint32_t* edits, uint32_t edit_cap, uint32_t* n_edits) {
+    oracle::Graph g(ix);
+    const oracle::wfa::Alignment a = run_wfa(g, scores, error_model, mode, seq, seq_len, from_node, from_offset, to_node, to_offset, nullptr);
     *ok = a.ok ? 1 : 0; *score = a.score; *node_offset = a.node_offset; *seq_offset = a.seq_offset; *length = a.length;
     if (a.path.size() > path_cap || a.edits.size() > edit_cap) return -1;
     for (size_t i = 0; i < a.path.size(); i++) path[i] = a.path[i];
     for (size_t i = 0; i < a.edits.size(); i++) edits[i] = (a.edits[i].second << 2) | (uint32_t)a.edits[i].first;
     *n_path = (uint32_t)a.path.size(); *n_edits = (uint32_t)a.edits.size();
     return 0;
+}
+
+// The same problem as oracle_wfa, reporting what gb_wfa_batch's per-problem workspace needs for it.  out[11]:
+// trie nodes, sequence bytes, path entries, wavefront points (all matrices and trie nodes), distinct possible scores,
+// largest point score, smallest and largest point diagonal, largest point seq offset and node offset, most successors
+// met in one expansion.  All zero when the start position is not in the graph (nothing is aligned).
+extern "C" void oracle_wfa_workspace(const gb_flat_index* ix, const gb_scores* scores, const double* error_model, int mode,
+                                     const uint8_t* seq, uint32_t seq_len, uint32_t from_node, uint32_t from_offset, uint32_t to_node, uint32_t to_offset,
+                                     int32_t* out) {
+    oracle::Graph g(ix);
+    oracle::wfa::Workspace w;
+    run_wfa(g, scores, error_model, mode, seq, seq_len, from_node, from_offset, to_node, to_offset, &w);
+    const int32_t v[11] = {(int32_t)w.trie_nodes, (int32_t)w.seq_bytes, (int32_t)w.path_entries, (int32_t)w.points, (int32_t)w.scores,
+                           w.max_score, w.min_diagonal, w.max_diagonal, (int32_t)w.max_seq_offset, (int32_t)w.max_node_offset, (int32_t)w.max_successors};
+    for (int i = 0; i < 11; i++) out[i] = v[i];
 }

@@ -744,10 +744,12 @@ class Device:
                                    for c in range(int(nch[p]))]})
         return out
 
-    def wfa_batch(self, problems, error_model=None, path_cap=512, edit_cap=512):
+    def wfa_batch(self, problems, error_model=None, path_cap=512, edit_cap=512, with_status=False):
         """gb_wfa_batch.  problems: list of (mode, sequence bytes, (from node, from offset) or None,
         (to node, to offset) or None) with mode 0 connect / 1 suffix / 2 prefix and oriented nodes.
-        Returns list of dicts with the WFAAlignment fields (edits as (op letter, length), ops "MXID")."""
+        Returns list of dicts with the WFAAlignment fields (edits as (op letter, length), ops "MXID"),
+        every problem asserted to fit the workspace and caps; with_status=True returns "ok" as the
+        kernel's -1 / 0 / 1 instead."""
         lib = load_library()
         n = len(problems)
         seq_off = np.zeros(n + 1, dtype=np.uint64)
@@ -765,8 +767,8 @@ class Device:
             raise GbError(rc, "gb_wfa_batch")
         out = []
         for i in range(n):
-            assert ok[i] >= 0, f"problem {i}: workspace capacity exceeded"
-            out.append({"ok": bool(ok[i]), "score": int(score[i]), "node_offset": int(noff[i]), "seq_offset": int(soff[i]), "length": int(length[i]),
+            assert with_status or ok[i] >= 0, f"problem {i}: workspace capacity exceeded"
+            out.append({"ok": int(ok[i]) if with_status else bool(ok[i]), "score": int(score[i]), "node_offset": int(noff[i]), "seq_offset": int(soff[i]), "length": int(length[i]),
                         "path": [int(x) for x in path[i * path_cap: i * path_cap + int(npath[i])]],
                         "edits": [("MXID"[int(w) & 3], int(w) >> 2) for w in edits[i * edit_cap: i * edit_cap + int(nedits[i])]]})
         return out

@@ -407,19 +407,6 @@ __device__ inline void wfa_connect(const DevIndex& ix, const DevScores& sc, cons
     out.node_offset = from_offset + 1; out.seq_offset = 0;
     out.length = P.cand_seq_offset + unaligned_tail;
     out.score = (sc.match * ((int32_t)(P.cand_seq_offset + unaligned_tail) + ((int32_t)P.cand_seq_offset - P.cand_diagonal)) - P.cand_score) / 2;
-    // the graph path of the candidate's trie branch, root first
-    {
-        uint32_t total = 0;
-        for (uint32_t node = P.cand_node;; node = ws.nodes[node].parent) { total += ws.nodes[node].path_len; if (node == 0) break; }
-        if (total > path_cap) { out.ok = -1; return; }
-        uint32_t w = total;
-        for (uint32_t node = P.cand_node;; node = ws.nodes[node].parent) {
-            const WfaNode n = ws.nodes[node];
-            for (uint32_t i = n.path_len; i > 0; i--) out_path[--w] = ws.path[n.path_off + i - 1];
-            if (node == 0) break;
-        }
-        out.n_path = total;
-    }
     // backtrace; edits appended (merged) in reverse order
     uint32_t ne = 0;
     auto append = [&](uint32_t op, uint32_t len) {
@@ -467,17 +454,33 @@ __device__ inline void wfa_connect(const DevIndex& ix, const DevScores& sc, cons
     if (out.ok != 1) return;
     for (uint32_t i = 0; i < ne / 2; i++) { const uint32_t t = out_edits[i]; out_edits[i] = out_edits[ne - 1 - i]; out_edits[ne - 1 - i] = t; }
     out.n_edits = ne;
-    // drop an unused first node, then unused trailing nodes (gbwt_extender.cpp:2191-2212)
-    uint32_t p0 = 0, pn = out.n_path;
-    if (pn > 0 && out.node_offset >= load_node(ix, out_path[0]).len) { p0 = 1; out.node_offset = 0; }
-    int64_t final_offset = out.node_offset;
-    for (uint32_t i = 0; i < ne; i++) if ((out_edits[i] & 3u) != W_INSERTION) final_offset += out_edits[i] >> 2;
-    for (uint32_t i = p0; i + 1 < pn; i++) final_offset -= load_node(ix, out_path[i]).len;
-    while ((pn - p0 == 1 && final_offset == (int64_t)out.node_offset) || (pn - p0 > 1 && final_offset <= 0)) {
-        pn--;
-        if (pn > p0) final_offset += load_node(ix, out_path[pn - 1]).len;
+    // The graph path is the candidate's trie branch, root first, without an unused first node and unused trailing
+    // nodes (gbwt_extender.cpp:2191-2212).  A trie node grows along a non-branching haplotype up to WFA_TARGET_LENGTH
+    // bases, so the branch can run far past the alignment: the kept range [p0, pn) is found first, walking the branch
+    // from its end, and only that range has to fit path_cap.
+    uint32_t total = 0; int64_t branch_len = 0;
+    for (uint32_t node = P.cand_node;; node = ws.nodes[node].parent) {
+        total += ws.nodes[node].path_len; branch_len += ws.nodes[node].seq_len;
+        if (node == 0) break;
     }
-    if (p0) for (uint32_t i = p0; i < pn; i++) out_path[i - p0] = out_path[i];
+    const uint32_t from_len = load_node(ix, from_node).len;          // the root's first graph node
+    const uint32_t p0 = out.node_offset >= from_len ? 1u : 0u;
+    if (p0) out.node_offset = 0;
+    uint32_t pn = total;
+    uint32_t c = P.cand_node, ci = ws.nodes[c].path_len;              // cursor: entry ci - 1 of trie node c is branch entry pn - 1
+    auto step_back = [&]() { if (--ci == 0 && c != 0) { c = ws.nodes[c].parent; ci = ws.nodes[c].path_len; } };
+    auto entry = [&]() { return ws.path[ws.nodes[c].path_off + ci - 1]; };
+    if (pn > p0) {
+        int64_t final_offset = out.node_offset;
+        for (uint32_t i = 0; i < ne; i++) if ((out_edits[i] & 3u) != W_INSERTION) final_offset += out_edits[i] >> 2;
+        final_offset -= branch_len - (p0 ? from_len : 0u) - load_node(ix, entry()).len;
+        while ((pn - p0 == 1 && final_offset == (int64_t)out.node_offset) || (pn - p0 > 1 && final_offset <= 0)) {
+            pn--; step_back();
+            if (pn > p0) final_offset += load_node(ix, entry()).len;
+        }
+    }
+    if (pn - p0 > path_cap) { out.ok = -1; return; }
+    for (uint32_t i = pn; i > p0; i--, step_back()) out_path[i - 1 - p0] = entry();
     out.n_path = pn - p0;
 }
 

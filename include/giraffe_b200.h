@@ -539,7 +539,9 @@ int gb_plan_stats(gb_device* dev, uint64_t* out4);
  * index, a first node whose parent is not negative, a later node whose parent is negative (a
  * second root), not below its own index or not on the path from the root to the node before
  * it (not DFS visit order), a root_trim not below the root's length, or a node 512 or more
- * levels below the root.
+ * levels below the root; or when a max_gap is above 65535 (vg's max_gap is a uint16_t).
+ * A max_gap of 0 is taken as 1: the leading insertion may then be one base long and the
+ * X-drop threshold is gap_open.
  * ---------------------------------------------------------------------------------- */
 int gb_xdrop_pinned_batch(gb_device* dev, uint32_t n,
                           const int32_t* tree_parent, const uint32_t* tree_node, const uint64_t* tree_off,
@@ -560,7 +562,14 @@ int gb_xdrop_pinned_batch(gb_device* dev, uint32_t n,
  * bonus is granted at each read end that is aligned rather than soft clipped.
  * Outputs per problem: score (0 and no mappings when nothing scores > 0), mappings
  * (node = index into the problem's node list), edits (soft clips are insertions on the first /
- * last mapping), counts, status.
+ * last mapping), counts, status: GB_ITEM_OUT_FULL when the path exceeds map_cap / edit_cap,
+ * with score 0 and both counts 0.
+ * The three DAG seams (gb_sw_batch, gb_banded_global_batch, gb_xdrop_dag_batch) return
+ * GB_ERR_ARG, before anything is uploaded, when map_cap or edit_cap is 0, a query is longer
+ * than 1024 bases, a problem has 2^24 or more nodes (traceback steps carry the node index in
+ * 24 bits), a node id is below 2, not in the index or has no sequence, a node has more than 255
+ * predecessors, or a predecessor index is not below its node's; and GB_ERR_CAPACITY when the
+ * batch needs more than 8 GiB of traceback (one byte per base and query prefix).
  * ---------------------------------------------------------------------------------- */
 int gb_sw_batch(gb_device* dev, uint32_t n,
                 const uint32_t* node, const uint64_t* node_off, const uint32_t* pred, const uint64_t* pred_off,
@@ -579,7 +588,8 @@ int gb_sw_batch(gb_device* dev, uint32_t n,
  * Scoring: gb_set_scores without the full-length bonus; a pair with a non-ACGT base scores 0.
  * Outputs per problem: score, mappings (node = index into the problem's node list, every offset 0),
  * edits, counts, status: GB_ITEM_NO_BAND when no global alignment fits the band (nothing written),
- * GB_ITEM_OUT_FULL when the path exceeds map_cap / edit_cap.  An empty query is a deletion of the
+ * GB_ITEM_OUT_FULL when the path exceeds map_cap / edit_cap (score 0 and both counts 0; the input
+ * checks are those of gb_sw_batch, plus band_padding >= 0).  An empty query is a deletion of the
  * shortest source-to-sink path.  Rules and tie-breaking: oracle/banded_global.cpp.
  * ---------------------------------------------------------------------------------- */
 int gb_banded_global_batch(gb_device* dev, uint32_t n,
@@ -600,7 +610,14 @@ int gb_banded_global_batch(gb_device* dev, uint32_t n,
  * extension in attempt_rescue, minimizer_mapper.cpp:3345-3358).  Pass 1 extends the query suffix to
  * the right of the seed and fixes the head; pass 2 aligns the query prefix leftwards from the head
  * with traceback; the query right of the head is a soft clip.  score is the score of pass 2 (vg
- * rescores the path afterwards, fix_dozeu_score minimizer_mapper.cpp:3502).
+ * rescores the path afterwards, fix_dozeu_score minimizer_mapper.cpp:3502).  A max_gap of 0 is
+ * taken as 1, as in gb_xdrop_pinned_batch.  Status GB_ITEM_OUT_FULL when the path exceeds
+ * map_cap / edit_cap, with score 0 and both counts 0.
+ * Besides the checks of gb_sw_batch, returns GB_ERR_ARG before anything is uploaded when a max_gap
+ * is above 65535 (vg's max_gap is a uint16_t), a node has more than 255 successors, or a seed
+ * lies outside its problem: a seed node index not below the node count, a seed offset above the
+ * seed node's length or a seed query offset above the query length (an offset equal to the
+ * length is a seed at the end).
  * ---------------------------------------------------------------------------------- */
 int gb_xdrop_dag_batch(gb_device* dev, uint32_t n,
                        const uint32_t* node, const uint64_t* node_off, const uint32_t* pred, const uint64_t* pred_off,

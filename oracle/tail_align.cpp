@@ -72,6 +72,7 @@ PinnedAlignment xdrop_pinned(const Graph& g, const gb_scores& sc, const TailTree
     PinnedAlignment out;
     const size_t m = query.size(), n_nodes = tree.nodes.size();
     const int32_t go = sc.gap_open, ge = sc.gap_extend;
+    max_gap_length = std::max<uint32_t>(max_gap_length, 1);         // a max_gap of 0 means 1, as in the kernels
     const int32_t xt = go + ge * ((int32_t)max_gap_length - 1);   // cost of the longest allowed gap
     struct NodeDP {
         std::string seq;

@@ -52,6 +52,7 @@ PassResult xdrop_dag_pass(const OrientedDag& dag, const gb_scores& sc, const std
     PassResult out;
     const size_t N = dag.seq.size(), m = query.size(), W = m + 1;
     const int32_t go = sc.gap_open, ge = sc.gap_extend;
+    max_gap = std::max<uint32_t>(max_gap, 1);                       // a max_gap of 0 means 1, as in the kernels
     const int32_t xt = go + ge * ((int32_t)max_gap - 1);
     struct NodeDP { std::vector<int32_t> H, E, F, inH, inE; std::vector<int32_t> argH, argE; int32_t lineage_max = 0; bool computed = false; bool live = false; uint32_t first_col = 0; };
     std::vector<NodeDP> dp(N);

@@ -53,7 +53,7 @@ def test_oracle_xdrop_matches_reference_vectors(case):
     index = case_index(case)
     sc = capi.Scores(*case["scores"])
     nodes = [2 * (i + 1) for i in range(len(case["nodes"]))]
-    score, path = oracle_xdrop(index, case["parents"], nodes, 0, case["read"], sc, max(case["max_gap"], 1))
+    score, path = oracle_xdrop(index, case["parents"], nodes, 0, case["read"], sc, case["max_gap"])
     want = case["score"] if "score" in case else eval(case["score_expr"], {"len": len(case["read"])})
     assert score == want
     if "path" in case:
@@ -117,8 +117,8 @@ def test_cuda_xdrop_matches_reference_vectors_and_oracle():
         index = case_index(case)
         dev = capi.Device(index, scores=capi.Scores(*case["scores"]))
         nodes = [2 * (i + 1) for i in range(len(case["nodes"]))]
-        got = dev.xdrop_pinned_batch([(case["parents"], nodes, 0, case["read"].encode(), max(case["max_gap"], 1))])[0]
-        want = oracle_xdrop(index, case["parents"], nodes, 0, case["read"], capi.Scores(*case["scores"]), max(case["max_gap"], 1))
+        got = dev.xdrop_pinned_batch([(case["parents"], nodes, 0, case["read"].encode(), case["max_gap"])])[0]
+        want = oracle_xdrop(index, case["parents"], nodes, 0, case["read"], capi.Scores(*case["scores"]), case["max_gap"])
         assert got[0] == want[0] and got[1] == want[1], case["name"]
         exp = case["score"] if "score" in case else eval(case["score_expr"], {"len": len(case["read"])})
         assert got[0] == exp

@@ -256,8 +256,8 @@ def eligible(pool, p, sc):
 
 # ---- GPU plumbing -------------------------------------------------------------------------------------------------
 def oracle_xdrop(index, p, scores):
-    """The oracle's pinned X-drop, outputs sized 1024 mappings / 4096 edits (the kernels clamp max_gap to 1).  Its
-    mappings name tree index + 1, as Device.xdrop_pinned_batch reports them."""
+    """The oracle's pinned X-drop, outputs sized 1024 mappings / 4096 edits.  Its mappings name tree index + 1, as
+    Device.xdrop_pinned_batch reports them."""
     lib = H.oracle_lib()
     parents, nodes, trim, q, gap = p
     par = np.asarray(parents, dtype=np.int32)
@@ -267,7 +267,7 @@ def oracle_xdrop(index, p, scores):
     maps = np.zeros(1024, dtype=H.mapping_dt)
     edits = np.zeros(4096, dtype=np.uint32)
     rc = lib.oracle_xdrop_pinned(C.byref(index.view), C.byref(scores), capi.ptr(par), capi.ptr(nd), len(nd), trim,
-                                 capi.ptr(qb), len(q), max(gap, 1), C.byref(score), capi.ptr(maps), 1024, C.byref(nm),
+                                 capi.ptr(qb), len(q), gap, C.byref(score), capi.ptr(maps), 1024, C.byref(nm),
                                  capi.ptr(edits), 4096, C.byref(ne))
     assert rc == 0
     return score.value, capi.decode_path(maps, edits, nm.value)

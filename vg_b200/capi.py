@@ -276,6 +276,22 @@ def _seam_outputs(n, map_cap, edit_cap):
             np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint8))
 
 
+def _dag_seam_results(outs, map_cap, with_status):
+    """The per-problem (score, path) of gb_sw_batch / gb_xdrop_dag_batch, every status asserted GB_ITEM_OK, or with
+    with_status (status, score, path) with the path decoded from the returned counts whatever the status."""
+    score, maps, edits, nm, _, status = outs
+    edit_cap = len(edits) // len(score)
+    res = []
+    for i in range(len(score)):
+        path = decode_path(maps[i * map_cap:], edits[i * edit_cap:], min(int(nm[i]), map_cap))
+        if with_status:
+            res.append((int(status[i]), int(score[i]), path))
+        else:
+            assert status[i] == GB_ITEM_OK, f"problem {i}: status {status[i]}"
+            res.append((int(score[i]), path))
+    return res
+
+
 class GbError(RuntimeError):
     def __init__(self, code: int, what: str):
         msg = load_library().gb_last_error()
@@ -637,22 +653,20 @@ class Device:
             out.append((int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i], node_offset=1)))
         return out
 
-    def sw_batch(self, problems, map_cap=512, edit_cap=2048):
+    def sw_batch(self, problems, map_cap=512, edit_cap=2048, with_status=False):
         """gb_sw_batch.  problems: list of (nodes, preds, query bytes) with nodes = oriented node ids in
         topological order and preds = per-node lists of predecessor indices.
-        Returns list of (score, [[problem_index, offset, [[op, len, base], ...]], ...])."""
+        Returns list of (score, [[problem_index, offset, [[op, len, base], ...]], ...]), every status
+        asserted GB_ITEM_OK; with_status=True returns (status, score, path) instead, path decoded from the
+        returned counts whatever the status."""
         lib = load_library()
         n = len(problems)
         dags = _pack_dags(problems)
-        score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
+        outs = _seam_outputs(n, map_cap, edit_cap)
         rc = lib.gb_sw_batch(self._h, n, *map(ptr, dags), map_cap, edit_cap, *map(ptr, outs))
         if rc != GB_OK:
             raise GbError(rc, "gb_sw_batch")
-        out = []
-        for i in range(n):
-            assert status[i] == GB_ITEM_OK, f"problem {i}: status {status[i]}"
-            out.append((int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i])))
-        return out
+        return _dag_seam_results(outs, map_cap, with_status)
 
     def banded_global_batch(self, problems, map_cap=512, edit_cap=2048):
         """gb_banded_global_batch.  problems: list of (nodes, preds, query bytes, band_padding, permissive)
@@ -670,24 +684,21 @@ class Device:
             raise GbError(rc, "gb_banded_global_batch")
         return [(int(status[i]), int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i])) for i in range(n)]
 
-    def xdrop_dag_batch(self, problems, map_cap=512, edit_cap=2048):
+    def xdrop_dag_batch(self, problems, map_cap=512, edit_cap=2048, with_status=False):
         """gb_xdrop_dag_batch.  problems: list of (nodes, preds, query bytes, seed or None, max_gap) with
-        seed = (node index, node offset, query offset).  Returns list of (score, path) like sw_batch."""
+        seed = (node index, node offset, query offset).  Returns list of (score, path) like sw_batch, and
+        with_status=True (status, score, path) like sw_batch."""
         lib = load_library()
         n = len(problems)
         seed = np.array([(0xFFFFFFFF, 0, 0) if p[3] is None else p[3] for p in problems], dtype=np.uint32).reshape(-1)
         gap = np.array([p[4] for p in problems], dtype=np.uint32)
         dags = _pack_dags(problems)
-        score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
+        outs = _seam_outputs(n, map_cap, edit_cap)
         rc = lib.gb_xdrop_dag_batch(self._h, n, *map(ptr, dags), ptr(seed), ptr(gap), map_cap, edit_cap,
                                     *map(ptr, outs))
         if rc != GB_OK:
             raise GbError(rc, "gb_xdrop_dag_batch")
-        out = []
-        for i in range(n):
-            assert status[i] == GB_ITEM_OK, f"problem {i}: status {status[i]}"
-            out.append((int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i])))
-        return out
+        return _dag_seam_results(outs, map_cap, with_status)
 
     def chain_candidates_batch(self, problems, limit=2 ** 64 - 1, cap=None):
         """gb_chain_candidates_batch.  problems: list of seed lists [(oriented node, offset), ...].

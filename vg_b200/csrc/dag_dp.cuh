@@ -252,7 +252,6 @@ __device__ inline void xd_align(const DevIndex& ix, const DevScores& sc, const D
     // ---- pass 1: the head ---------------------------------------------------------------------------
     uint32_t head_u, head_off, head_q;
     if (seed_u != 0xffffffffu) {
-        if (seed_u >= N || seed_q > m || seed_o > v.seq_len[seed_u]) { status = GB_ITEM_OUT_FULL; return; }
         const uint32_t m1 = m - seed_q;
         for (uint32_t i = lane; i < m1; i += 32) q[i] = dp_query_base(query[seed_q + i]);
         __syncwarp();

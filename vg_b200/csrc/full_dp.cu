@@ -51,7 +51,8 @@ sw_kernel(DevIndex ix, DevScores sc, SwBatch b) {
             const uint8_t* read = b.dag.read(p, m);
             sw_align(ix, sc, v, read, m, q, dps, score, out, status);
         }
-        b.out.store(p, status == GB_ITEM_OK ? score : 0, out.n_maps, out.n_edits, status);
+        const bool ok = status == GB_ITEM_OK;
+        b.out.store(p, ok ? score : 0, ok ? out.n_maps : 0, ok ? out.n_edits : 0, status);
         __syncwarp();
     }
 }

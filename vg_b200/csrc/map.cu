@@ -943,7 +943,8 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
         max_q = std::max<uint32_t>(max_q, (uint32_t)(query_off[i + 1] - query_off[i]));
         const uint64_t t0 = tree_off[i]; const uint32_t ntree = (uint32_t)(tree_off[i + 1] - t0);
         if (ntree == 0) return fail("empty tree");
-        lineage.clear();                      // root .. previous node
+        if (max_gap[i] > 65535) return fail("max_gap above 65535");      // vg's max_gap is a uint16_t
+        lineage.clear();                     // root .. previous node
         for (uint32_t x = 0; x < ntree; x++) {
             const uint32_t v = tree_node[t0 + x]; const int32_t par = tree_parent[t0 + x];
             if (v < 2 || v >= d->ix.n_nodes || d->h_node_len[v] == 0) return fail("unknown node");

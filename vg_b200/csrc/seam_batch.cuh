@@ -108,8 +108,8 @@ struct DagProblems {
                 const uint8_t* query_, const uint64_t* query_off_)
         : n(n_), node(node_), node_off(node_off_), pred(pred_), pred_off(pred_off_), query(query_), query_off(query_off_) {}
 
-    // Refuses unknown nodes, nodes with more than 255 predecessors and predecessors that do not precede their
-    // node; sizes the workspaces.
+    // Refuses problems of 2^24 or more nodes, unknown nodes (ids out of range or without sequence), nodes with more
+    // than 255 predecessors and predecessors that do not precede their node; sizes the workspaces.
     int validate(const gb_device* d, const char* who) {
         total_nodes = node_off[n];
         m.assign(n, 0); N.assign(n, 0); bases.assign(n, 0);
@@ -118,10 +118,12 @@ struct DagProblems {
             m[p] = (uint32_t)(query_off[p + 1] - query_off[p]);
             max_q = std::max(max_q, m[p]);
             N[p] = node_off[p + 1] - node_off[p];
+            // traceback steps carry the node index in 24 bits
+            if (N[p] >= (1u << 24)) return fail(who, ": more than 2^24 - 1 nodes in a problem");
             for (uint64_t u = 0; u < N[p]; u++) {
                 const uint64_t g = node_off[p] + u;
                 const uint32_t v = node[g];
-                if (v < 2 || v >= d->ix.n_nodes) return fail(who, ": unknown node");
+                if (v < 2 || v >= d->ix.n_nodes || d->h_node_len[v] == 0) return fail(who, ": unknown node");
                 if (pred_off[g + 1] - pred_off[g] > 255) return fail(who, ": more than 255 predecessors");
                 for (uint64_t e = pred_off[g]; e < pred_off[g + 1]; e++)
                     if (pred[e] >= u) return fail(who, ": nodes are not in topological order");

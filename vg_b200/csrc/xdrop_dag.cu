@@ -76,6 +76,16 @@ extern "C" int gb_xdrop_dag_batch(gb_device* d, uint32_t n,
     DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
     int rc;
     if ((rc = dag.validate(d, "gb_xdrop_dag_batch"))) return rc;
+    for (uint32_t p = 0; p < n; p++) {
+        // vg's max_gap is a uint16_t (DozeuInterface::align), and the X-drop threshold go + ge * (max_gap - 1) is int32
+        if (max_gap[p] > 65535) return DagProblems::fail("gb_xdrop_dag_batch", ": max_gap above 65535");
+        // a seed lies in its problem: a node of the list, an offset up to that node's length, a query offset up to m
+        const uint32_t su = seed[3 * p], so = seed[3 * p + 1], sq = seed[3 * p + 2];
+        if (su == 0xffffffffu) continue;
+        if (su >= dag.N[p]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed node outside the problem");
+        if (so > d->h_node_len[node[node_off[p] + su]]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed offset past the seed node");
+        if (sq > dag.m[p]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed query offset past the query");
+    }
     // successor CSR, ascending (nodes are visited in ascending order), at most 255 successors per node
     const uint64_t total_pred = pred_off[dag.total_nodes];
     std::vector<uint64_t> succ_off(dag.total_nodes + 1, 0);

@@ -363,11 +363,9 @@ __device__ inline bool fast_read(const DevIndex& ix, const MapParamsDev& P, cons
 
 struct FastArgs { uint32_t* slow_list; uint32_t* slow_count; };
 
-// MINB != 0 caps the registers for that many resident blocks per SM, which makes the kernel spill to local memory.  Measured
-// on an H100 SXM at a 400 W power limit, per 1 M reads (500 k pairs) of config 2: uncapped 7.4 ms, 12 blocks 16.4 ms, 16 blocks 18.7 ms.
-// GIRAFFE_B200_FAST_MINB = 0 | 12 | 16 picks the instantiation; 0 (uncapped) is the default
-template <int MINB>
-__global__ void __launch_bounds__(128, MINB ? MINB : 1)
+// Registers uncapped: a cap for 12 or 16 resident blocks per SM makes the kernel spill to local memory.  Measured on an
+// H100 SXM at a 400 W power limit, per 1 M reads (500 k pairs) of config 2: uncapped 7.4 ms, 12 blocks 16.4 ms, 16 blocks 18.7 ms.
+__global__ void __launch_bounds__(128, 1)
 align_fast_kernel_pe(DevIndex ix, MapParamsDev P, DevScores sc, MapBatch b, AlignArgs a, FastArgs fa) {
     const uint32_t n_pairs = b.n_reads / 2;
     for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n_pairs; p += gridDim.x * blockDim.x) {

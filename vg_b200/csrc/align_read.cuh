@@ -32,6 +32,31 @@ struct AlignArgs {
 constexpr uint32_t N_SLOTS = 2 * MAX_CANDS + 8 + 32;   // candidate path slots per warp (both mates of a pair, + rescued alignments)
 constexpr uint32_t N_TEMP_SLOTS = 5;              // res_left, res_right, scratch, middle, assembly
 
+// Dynamic shared memory per warp of the warp-per-unit align kernels (align_kernel: 1 mate, align_kernel_pe: 2): the reads
+// of the unit's mates, their qualities and the query buffer (Lc bytes each, rounded up to 16 together), the four DP
+// columns of Lc + 1 cells and 64 spare bytes, then tmp_bytes for the temporary path slots.  Lc is a multiple of 16, so
+// from the query buffer on this is the layout of dp_smem_per_warp(Lc).
+__host__ __device__ inline size_t align_bytes_part(uint32_t Lc, uint32_t mates) { return ((size_t)(2 * mates + 1) * Lc + 15) & ~(size_t)15; }
+__host__ __device__ inline size_t align_smem_per_warp(uint32_t Lc, uint32_t mates, uint32_t tmp_bytes) {
+    return align_bytes_part(Lc, mates) + (size_t)(Lc + 1) * 4 * 4 + 64 + tmp_bytes;
+}
+struct AlignSmem {
+    uint8_t* tmp;                                  // nullptr when tmp_bytes is 0
+    uint8_t* read[2]; uint8_t* qual[2];            // [mate]
+    uint8_t* qbuf;
+    DpSmem dps;
+};
+__device__ inline AlignSmem align_smem_carve(uint8_t* smem, int warp, uint32_t Lc, uint32_t mates, uint32_t tmp_bytes) {
+    uint8_t* base = smem + (size_t)warp * align_smem_per_warp(Lc, mates, tmp_bytes);
+    AlignSmem s;
+    s.tmp = tmp_bytes ? base + align_bytes_part(Lc, mates) + (size_t)(Lc + 1) * 4 * 4 + 64 : nullptr;
+    s.read[0] = base; s.read[1] = base + Lc;                                 // read[1], qual[1]: two mates only
+    s.qual[0] = base + (size_t)mates * Lc; s.qual[1] = base + (size_t)(mates + 1) * Lc;
+    s.qbuf = base + 2 * (size_t)mates * Lc;
+    s.dps = dp_cols_carve(reinterpret_cast<int32_t*>(base + align_bytes_part(Lc, mates)), Lc);
+    return s;
+}
+
 // (real calls: the FP64 log1p / exp bodies are several hundred instructions and the align kernels are instruction-fetch bound)
 static __device__ __noinline__ double d_add_log(double x, double y) { return x > y ? x + log1p(exp(y - x)) : y + log1p(exp(x - y)); }
 static __device__ __noinline__ double d_subtract_log(double x, double y) { return x + log1p(-exp(y - x)); }

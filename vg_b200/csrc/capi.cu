@@ -46,10 +46,9 @@ struct ExtendBatch {
     uint32_t* post_list; uint32_t* post_count; uint32_t* post_work;
 };
 
-// MINB: resident blocks per SM the register budget is cut for (6: 40 registers, 5: 48, 4: 64, 3: 80, 2: 128); GIRAFFE_B200_EXTEND_MINB picks
-// the instantiation at run time (tuning knob; default 4)
-template <int MINB>
-__global__ void __launch_bounds__(EXTEND_WARPS * 32, MINB)
+// Four resident blocks per SM (a 64-register budget).  Measured on an H100 (DESIGN.md §5): 3 blocks 7.2 ms, 4 blocks 7.0 ms,
+// 5 blocks 11.8 ms.
+__global__ void __launch_bounds__(EXTEND_WARPS * 32, 4)
 extend_kernel(DevIndex ix, ExtendParams p, ExtendBatch b, ExtendWorkspace ws) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int warp_in_block = threadIdx.x >> 5;
@@ -169,8 +168,6 @@ extern "C" int gb_device_create(const gb_flat_index* ix, int device_ordinal, gb_
         if (v >= 2 && v <= (1ul << 24)) d->map_chunk = (uint32_t)(v & ~1ul);
     }
     if (const char* env = std::getenv("GIRAFFE_B200_TILES")) d->use_tiles = std::atoi(env) != 0;
-    if (const char* env = std::getenv("GIRAFFE_B200_EXTEND_MINB")) { const int v = std::atoi(env); if (v >= 2 && v <= 6) d->extend_minb = v; }
-    if (const char* env = std::getenv("GIRAFFE_B200_FAST_MINB")) { const int v = std::atoi(env); if (v == 0 || v == 12 || v == 16) d->fast_minb = v; }
     if (const char* env = std::getenv("GIRAFFE_B200_POOL_SCALE")) {
         const double v = std::strtod(env, nullptr);
         if (v > 0.0 && v <= 1024.0) d->pool_scale = v;
@@ -244,7 +241,6 @@ extern "C" void gb_device_destroy(gb_device* d) {
     if (!d) return;
     cudaSetDevice(d->device);
     cudaStreamSynchronize(d->stream);
-    d->release_all();
     for (int i = 0; i < 5; i++) cudaEventDestroy(d->ev_stage[i]);
     cudaFree(d->work_counter);
     cudaEventDestroy(d->ev0); cudaEventDestroy(d->ev1);
@@ -252,10 +248,11 @@ extern "C" void gb_device_destroy(gb_device* d) {
         cudaEventDestroy(d->io[i].ev_in); cudaEventDestroy(d->io[i].ev_done); cudaEventDestroy(d->io[i].ev_hdr);
         cudaEventDestroy(d->io[i].ev_out); cudaEventDestroy(d->io[i].ev_k0); cudaEventDestroy(d->io[i].ev_k1);
     }
+    for (cudaEvent_t ev : d->kt_ev) if (ev) cudaEventDestroy(ev);
     cudaFreeHost(d->h_totals);
     cudaStreamDestroy(d->s_in); cudaStreamDestroy(d->s_out);
     cudaStreamDestroy(d->own_stream);
-    delete d;
+    delete d;                              // the DevBuf destructors free the device memory
 }
 
 extern "C" int gb_set_scores(gb_device* d, const gb_scores* s) {
@@ -276,14 +273,12 @@ int launch_extend(gb_device* d, const ExtendParams& p, const ExtendBatch& b_in, 
     if (b.read_cap == 0) b.read_cap = 16;
     const size_t smem = (size_t)EXTEND_WARPS * b.read_cap;
     if (smem > 200 * 1024) { g_last_error = "read too long for the extension kernel"; return GB_ERR_ARG; }
-    const int minb = d->extend_minb;
-    auto kern = minb == 2 ? extend_kernel<2> : (minb == 3 ? extend_kernel<3> : (minb == 5 ? extend_kernel<5> : (minb == 6 ? extend_kernel<6> : extend_kernel<4>)));
     if (smem > 48 * 1024) {
-        GB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        GB_CUDA(cudaFuncSetAttribute(extend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         GB_CUDA(cudaFuncSetAttribute(extend_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     int blocks_per_sm = 0;
-    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, EXTEND_WARPS * 32, smem));
+    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, extend_kernel, EXTEND_WARPS * 32, smem));
     if (blocks_per_sm < 1) blocks_per_sm = 1;
     uint32_t grid = (uint32_t)(d->n_sms * blocks_per_sm);
     const uint32_t needed = (b.n_items + EXTEND_WARPS - 1) / EXTEND_WARPS;
@@ -296,7 +291,7 @@ int launch_extend(gb_device* d, const ExtendParams& p, const ExtendBatch& b_in, 
     ExtendWorkspace ws{d->ws_queue.ptr, d->ws_arena.ptr, EXTEND_Q_CAP, EXTEND_A_CAP};
     b.work_counter = d->work_counter; b.post_list = d->p_post.ptr; b.post_count = d->work_counter + 1; b.post_work = d->work_counter + 2;
     GB_CUDA(cudaMemsetAsync(d->work_counter, 0, 4 * sizeof(uint32_t), d->stream));
-    kern<<<grid, EXTEND_WARPS * 32, smem, d->stream>>>(d->ix, p, b, ws);
+    extend_kernel<<<grid, EXTEND_WARPS * 32, smem, d->stream>>>(d->ix, p, b, ws);
     d->launches++;
     GB_CUDA(cudaGetLastError());
     if (mark && (rc = d->kt_mark(b.in_list ? "extend_kernel(large strides)" : "extend_kernel"))) return rc;

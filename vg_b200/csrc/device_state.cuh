@@ -8,6 +8,7 @@
 namespace gb { struct DbgCluster; }
 
 #include <cuda_runtime.h>
+#include <cstddef>
 #include <string>
 #include <vector>
 
@@ -58,6 +59,31 @@ struct DevBuf {
     }
 };
 
+// The mapping pipeline's device counters, zeroed at the start of every map_device call: work counters that hand units
+// to the persistent kernels, and the cursors and counts of what the kernels appended to the pools and lists.  The
+// extension launches count on d->work_counter, so they have no field here.
+struct MapCursors {
+    uint32_t seed_work;                              // seeding, first pass
+    uint32_t min_cursor, seed_cursor, item_cursor, ext_cursor;      // SeedPools
+    uint32_t align_work;                             // align fast path, then the warp-per-unit align kernel
+    uint32_t slow_count;                             // units the fast path leaves to the warp-per-unit kernels
+    uint32_t seed_retry_count;                       // units the first seeding pass could not fit
+    uint32_t seed_retry_work;                        // seeding, second pass
+    uint32_t seed_retry_again;                       // units the second pass lists again (not read)
+    uint32_t rescue_count, rescue_work;              // pairs deferred to the rescue build of align_kernel_pe
+    uint32_t pool_overflow;                          // sticky: a pool ran out (the host doubles the pools and reruns)
+    uint32_t plan_work;                              // tail_plan_kernel
+    uint32_t big_ext_count;                          // items redone with the large extension strides
+    uint32_t tile_count, tile_units;                 // tiles, tile bytes / 16
+    uint32_t tile_list_count[2 * TILE_CLASSES];      // [wave][class]: tail_plan_kernel indexes it as one array
+    uint32_t tile_path_words;                        // result path pool of the tiles
+    uint32_t decide_work;                            // tail_decide_kernel
+    uint32_t tile_work[2 * TILE_CLASSES];            // [wave][class]
+};
+static_assert(sizeof(MapCursors) == 43 * sizeof(uint32_t), "MapCursors is 43 packed 32-bit counters");
+static_assert(offsetof(MapCursors, tile_path_words) == offsetof(MapCursors, tile_list_count) + 2 * TILE_CLASSES * sizeof(uint32_t),
+              "the two waves' tile list counts are contiguous");
+
 } // namespace gb
 
 struct gb_device {
@@ -95,7 +121,8 @@ struct gb_device {
     gb::DevBuf<gb::DevSeed> p_seeds;
     gb::DevBuf<gb::DevItem> p_items;
     gb::DevBuf<gb_seed> p_ext_seeds;
-    gb::DevBuf<uint32_t> p_cursors, p_ext_count, p_path, p_mism;
+    gb::DevBuf<gb::MapCursors> p_cursors;
+    gb::DevBuf<uint32_t> p_ext_count, p_path, p_mism;
     gb::DevBuf<uint8_t> p_ext_status;
     gb::DevBuf<uint32_t> p_big_list, p_big_of, p_big_path, p_big_mism; gb::DevBuf<gb_extension> p_big_ext;      // ExtendBig
     gb::DevBuf<gb_extension> p_ext;
@@ -117,7 +144,6 @@ struct gb_device {
         gb::DevBuf<gb_mapping> maps;
         gb::DevBuf<uint32_t> edits;
         cudaEvent_t ev_in = nullptr, ev_done = nullptr, ev_hdr = nullptr, ev_out = nullptr, ev_k0 = nullptr, ev_k1 = nullptr;
-        void release() { reads.release(); quals.release(); status.release(); read_off.release(); totals.release(); aln.release(); maps.release(); edits.release(); }
     } io[2];
     cudaStream_t s_in = nullptr, s_out = nullptr;
     uint64_t* h_totals = nullptr;          // pinned, 3 per set: mappings, edits, pool-overflow flag
@@ -126,7 +152,6 @@ struct gb_device {
     gb::DbgCluster* dbg_clusters = nullptr; bool debug_stop_after_seed = false;     // gb_debug_seed_stage
     // tail plan + DP tiles (xdrop_tile.cuh); GIRAFFE_B200_TILES=0 keeps every tail DP in the align kernels (int32 sweep)
     bool use_tiles = true; uint32_t last_tile_problems = 0;
-    int extend_minb = 4, fast_minb = 0;           // launch-bounds instantiations (GIRAFFE_B200_EXTEND_MINB / _FAST_MINB)
     gb_alignment* mirror_aln = nullptr; gb_mapping* mirror_maps = nullptr; uint32_t* mirror_edits = nullptr; uint64_t mirror_map_cap = 0, mirror_edit_cap = 0;
     gb::DevBuf<gb::TailPlanEntry> pl_entries;
     gb::DevBuf<uint32_t> pl_unit_base, pl_unit_count, pl_tile_off, pl_lists, pl_paths;
@@ -147,14 +172,4 @@ struct gb_device {
     }
     gb::DevBuf<uint64_t> c_run;            // running mapping / edit totals of a host-buffer call
     uint32_t map_chunk = 1u << 20;         // reads per chunk; GIRAFFE_B200_MAP_CHUNK overrides
-    void release_all() {
-        nodes.release(); seq.release(); gbwt.release(); dist.release(); table.release(); hits.release(); slot_order.release(); slots.release(); site_dist.release();
-        ws_queue.release(); ws_arena.release(); p_post.release();
-        t_hit.release(); t_plo.release(); t_phred.release(); p_states.release(); p_min.release(); p_seeds.release();
-        p_items.release(); p_ext_seeds.release(); p_cursors.release(); p_ext_count.release(); p_path.release(); p_mism.release();
-        p_ext_status.release(); p_ext.release(); p_big_list.release(); p_big_of.release(); p_big_path.release(); p_big_mism.release(); p_big_ext.release(); ws_tail.release(); ws_cand.release(); ws_rescue.release(); w_reads.release(); w_quals.release(); p_pairs.release(); p_slow.release(); p_rescue.release(); p_retry.release();
-        pad_maps.release(); pad_edits.release(); c_map_off.release(); c_edit_off.release(); c_totals.release(); c_tmp.release();
-        io[0].release(); io[1].release(); c_run.release();
-        pl_entries.release(); pl_unit_base.release(); pl_unit_count.release(); pl_tile_off.release(); pl_lists.release(); pl_paths.release(); pl_tiles.release(); ws_tile.release(); pl_results.release(); pl_stats.release();
-    }
 };

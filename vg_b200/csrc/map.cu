@@ -1,6 +1,12 @@
-// map.cu — gb_map_batch: the single-end Giraffe hot path on the GPU.
-//   seed_kernel -> extend_kernel -> align_kernel, all persistent warp-per-unit kernels pulling
-//   work from atomic counters; intermediate records stay in HBM (map_state.cuh).
+// map.cu — gb_map_batch / gb_map_paired_batch: the single- and paired-end Giraffe hot path on the GPU.
+//   map_device runs the stages of one batch (a chunk of the host-buffer entry points):
+//     seeding       seed_kernel / seed_kernel_pe (map_paired.cuh), then a second pass at the maximum table sizes
+//     extension     extend_kernel + extend_finish_kernel (capi.cu), then the repeats again with large strides
+//     align         align_fast_kernel(_pe) (align_fast.cuh), thread per unit; the units it cannot finish go on to
+//     tails         tail_plan_kernel, xdrop_tile_kernel per size class, tail_decide_kernel, tiles again (tail_plan.cuh)
+//                   and align_kernel / align_kernel_pe (+ its rescue build), warp per unit
+//     compaction    compact.cuh: the records packed into the caller's pools
+//   The persistent kernels pull work from the counters of MapCursors; intermediate records stay in HBM (map_state.cuh).
 // No CPU fallback: every stage is a CUDA kernel; the host only moves buffers and launches.
 #include <cub/cub.cuh>
 #include "giraffe_b200.h"
@@ -9,7 +15,6 @@
 #include "align.cuh"
 #include "extend.cuh"
 #include "dag_dp.cuh"
-#include "seam_batch.cuh"
 
 #include <algorithm>
 #include <cfloat>
@@ -97,14 +102,9 @@ align_kernel(DevIndex ix, MapParamsDev P, DevScores sc, MapBatch b, AlignArgs a)
     extern __shared__ __align__(16) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t gwarp = blockIdx.x * ALIGN_WARPS + warp;
-    const uint32_t W = b.Lc + 1;
-    // shared per warp: read, qual, query buffer, 4 DP columns
-    const size_t per_warp = ((size_t)b.Lc * 3 + 15 & ~(size_t)15) + (size_t)W * 4 * 4 + 64 + a.tmp_bytes;
-    uint8_t* base = smem + (size_t)warp * per_warp;
-    uint8_t* stmp = a.tmp_bytes ? base + (((size_t)b.Lc * 3 + 15) & ~(size_t)15) + (size_t)W * 4 * 4 + 64 : nullptr;
-    uint8_t* sread = base; uint8_t* squal = base + b.Lc; uint8_t* qbuf = base + 2 * (size_t)b.Lc;
-    int32_t* cols = reinterpret_cast<int32_t*>(base + (((size_t)b.Lc * 3 + 15) & ~(size_t)15));
-    DpSmem dps; dps.Hp = cols; dps.Ep = cols + W; dps.Hc = cols + 2 * W; dps.Ec = cols + 3 * W;
+    const AlignSmem sm = align_smem_carve(smem, warp, b.Lc, 1, a.tmp_bytes);
+    uint8_t* sread = sm.read[0]; uint8_t* squal = sm.qual[0]; uint8_t* qbuf = sm.qbuf; uint8_t* stmp = sm.tmp;
+    const DpSmem dps = sm.dps;
     const TailWs ws = carve_tail_ws(a.ws_base + (size_t)gwarp * a.ws_stride, b.Lc, a.tb_cells);
     uint8_t* cand_base = a.cand_base + (size_t)gwarp * a.cand_stride;
 
@@ -177,62 +177,69 @@ extern "C" void gb_map_params_default(gb_map_params* p) {
 
 namespace gb {
 
-// The three size classes of xdrop_tile_kernel over their work lists (lists[c * list_cap ..], counts on the device).
-template <int R>
-static int launch_tile_class(gb_device* d, int cls, const uint8_t* tiles, const uint32_t* tile_off, const uint32_t* lists, size_t list_cap,
-                             const uint32_t* list_count, uint32_t* work, TileResult* results, uint32_t* paths, uint32_t path_cap, uint32_t* path_cursor) {
-    const size_t smem = tile_smem_per_warp<R>() * TILE_WARPS;
-    GB_CUDA(cudaFuncSetAttribute(xdrop_tile_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int bps = 0;
-    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, xdrop_tile_kernel<R>, TILE_WARPS * 32, smem));
-    bps = std::max(1, std::min(bps, 2));
-    const uint32_t grid = (uint32_t)(d->n_sms * bps);
-    int rc;
-    if ((rc = d->ws_tile.reserve(tile_ws_bytes() * (size_t)d->n_sms * 2 * TILE_WARPS))) return rc;
-    TileBatch tb;
-    tb.tiles = tiles; tb.tile_off = tile_off; tb.list = lists + (size_t)cls * list_cap; tb.list_count = list_count + cls; tb.list_cap = (uint32_t)list_cap;
-    tb.work_counter = work + cls; tb.results = results; tb.path_pool = paths; tb.path_cap = path_cap; tb.path_cursor = path_cursor;
-    tb.ws_base = d->ws_tile.ptr; tb.ws_stride = tile_ws_bytes();
-    xdrop_tile_kernel<R><<<grid, TILE_WARPS * 32, smem, d->stream>>>(d->sc, tb);
-    d->launches++;
-    GB_CUDA(cudaGetLastError());
-    return d->kt_mark(R == 2 ? "xdrop_tile_kernel<2>" : R == 4 ? "xdrop_tile_kernel<4>" : R == 6 ? "xdrop_tile_kernel<6>" : R == 8 ? "xdrop_tile_kernel<8>" : R == 12 ? "xdrop_tile_kernel<12>" : "xdrop_tile_kernel<16>");
-}
+// xdrop_tile_kernel per size class c, which runs R = tile_class_rows(c) rows per lane.
+struct TileClassKernel { void (*kernel)(DevScores, TileBatch); size_t smem; const char* name; };
+static_assert(tile_class_rows(0) == 2 && tile_class_rows(1) == 4 && tile_class_rows(2) == 6 && tile_class_rows(3) == 8 &&
+              tile_class_rows(4) == 12 && tile_class_rows(5) == 16, "TILE_CLASS_KERNELS follows tile_class_rows");
+static const TileClassKernel TILE_CLASS_KERNELS[TILE_CLASSES] = {
+    {xdrop_tile_kernel<2>, tile_smem_per_warp<2>() * TILE_WARPS, "xdrop_tile_kernel<2>"},
+    {xdrop_tile_kernel<4>, tile_smem_per_warp<4>() * TILE_WARPS, "xdrop_tile_kernel<4>"},
+    {xdrop_tile_kernel<6>, tile_smem_per_warp<6>() * TILE_WARPS, "xdrop_tile_kernel<6>"},
+    {xdrop_tile_kernel<8>, tile_smem_per_warp<8>() * TILE_WARPS, "xdrop_tile_kernel<8>"},
+    {xdrop_tile_kernel<12>, tile_smem_per_warp<12>() * TILE_WARPS, "xdrop_tile_kernel<12>"},
+    {xdrop_tile_kernel<16>, tile_smem_per_warp<16>() * TILE_WARPS, "xdrop_tile_kernel<16>"},
+};
+
 int launch_tile_kernels(gb_device* d, const uint8_t* tiles, const uint32_t* tile_off, const uint32_t* lists, size_t list_cap,
                         const uint32_t* list_count, uint32_t* work, TileResult* results, uint32_t* paths, uint32_t path_cap, uint32_t* path_cursor) {
     int rc;
-    if ((rc = launch_tile_class<2>(d, 0, tiles, tile_off, lists, list_cap, list_count, work, results, paths, path_cap, path_cursor))) return rc;
-    if ((rc = launch_tile_class<4>(d, 1, tiles, tile_off, lists, list_cap, list_count, work, results, paths, path_cap, path_cursor))) return rc;
-    if ((rc = launch_tile_class<6>(d, 2, tiles, tile_off, lists, list_cap, list_count, work, results, paths, path_cap, path_cursor))) return rc;
-    if ((rc = launch_tile_class<8>(d, 3, tiles, tile_off, lists, list_cap, list_count, work, results, paths, path_cap, path_cursor))) return rc;
-    if ((rc = launch_tile_class<12>(d, 4, tiles, tile_off, lists, list_cap, list_count, work, results, paths, path_cap, path_cursor))) return rc;
-    return launch_tile_class<16>(d, 5, tiles, tile_off, lists, list_cap, list_count, work, results, paths, path_cap, path_cursor);
+    if ((rc = d->ws_tile.reserve(tile_ws_bytes() * (size_t)d->n_sms * 2 * TILE_WARPS))) return rc;
+    for (int cls = 0; cls < TILE_CLASSES; cls++) {
+        const TileClassKernel& k = TILE_CLASS_KERNELS[cls];
+        GB_CUDA(cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem));
+        int bps = 0;
+        GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k.kernel, TILE_WARPS * 32, k.smem));
+        bps = std::max(1, std::min(bps, 2));
+        TileBatch tb;
+        tb.tiles = tiles; tb.tile_off = tile_off; tb.list = lists + (size_t)cls * list_cap; tb.list_count = list_count + cls; tb.list_cap = (uint32_t)list_cap;
+        tb.work_counter = work + cls; tb.results = results; tb.path_pool = paths; tb.path_cap = path_cap; tb.path_cursor = path_cursor;
+        tb.ws_base = d->ws_tile.ptr; tb.ws_stride = tile_ws_bytes();
+        k.kernel<<<(uint32_t)(d->n_sms * bps), TILE_WARPS * 32, k.smem, d->stream>>>(d->sc, tb);
+        d->launches++;
+        GB_CUDA(cudaGetLastError());
+        if ((rc = d->kt_mark(k.name))) return rc;
+    }
+    return GB_OK;
 }
 
-// Device-resident mapping of a batch whose reads are already in HBM.
-int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
-               const uint64_t* d_read_off, uint32_t max_len, uint64_t total_bases,
-               gb_alignment* d_aln, uint8_t* d_status, bool paired,
-               gb_mapping* out_maps, uint64_t out_map_cap, uint32_t* out_edits, uint64_t out_edit_cap,
-               const uint64_t* d_run_base, uint32_t read_base, uint64_t* d_totals, uint32_t* d_overflow) {
-    int rc0;
-    if (hp->max_multimaps == 0 || hp->max_multimaps > GB_MAX_MULTIMAPS) { g_last_error = "max_multimaps must be 1 .. GB_MAX_MULTIMAPS"; return GB_ERR_ARG; }
-    // the seeding kernels pack (node id << 10 | offset) into 32 bits (DevSeed.id_off): node ids stop at 2^22 - 1
-    if (d->ix.n_nodes > (1u << 23)) { g_last_error = "the mapping kernels address node ids below 2^22 (4 194 303); split the graph (the stage seams have no such limit)"; return GB_ERR_CAPACITY; }
-    const uint32_t K = hp->max_multimaps;            // records per read, rank-major: record j * n_reads + read
-    if ((uint64_t)n_reads * K * std::max(hp->mapping_cap_per_read, hp->edit_cap_per_read) > 0xffffffffull) { g_last_error = "chunk too large for 32-bit record offsets (reads x max_multimaps x cap)"; return GB_ERR_ARG; }
-    if ((rc0 = d->pad_maps.reserve((size_t)n_reads * K * hp->mapping_cap_per_read))) return rc0;
-    if ((rc0 = d->pad_edits.reserve((size_t)n_reads * K * hp->edit_cap_per_read))) return rc0;
-    gb_mapping* d_maps = d->pad_maps.ptr; uint32_t* d_edits = d->pad_edits.ptr;
-    if (paired) {
-        if (n_reads % 2 != 0) { g_last_error = "paired mapping needs an even number of reads"; return GB_ERR_ARG; }
-        if (hp->max_rescue_attempts != 0 && hp->rescue_seed_limit >= RESCUE_SEEDS) { g_last_error = "rescue_seed_limit must be below 128"; return GB_ERR_ARG; }
-        if (!(hp->fragment_stdev > 0)) { g_last_error = "paired mapping needs a forced fragment length distribution"; return GB_ERR_ARG; }
-    }
-    const uint32_t Lc = std::max<uint32_t>(32u, (max_len + 15u) & ~15u);
-    if (Lc > 512) { g_last_error = "reads longer than 512 bp are not supported by the short-read path"; return GB_ERR_ARG; }
+// What the stages of one map_device call share.
+struct MapRun {
+    gb_device* d; const gb_map_params* hp;
+    uint32_t n_reads, n_units, K, Lc;          // n_units: reads, or pairs when paired
+    bool paired, rescue;
+    MapParamsDev P;
+    MapCursors* cur;
+    MapBatch b;                                // the reads as the kernels see them (paired: mate 2 rightward)
+    SeedPools pools;
+    size_t item_cap;
+    int32_t fragment_limit;
+    AlignArgs a;                               // ev from the extension stage, plan from the tail stage
+    // the warp-per-unit align kernels: the plain build (align_kernel or align_kernel_pe<false>), its grid, the grid of
+    // the rescue build, their dynamic shared memory
+    void (*align)(DevIndex, MapParamsDev, DevScores, MapBatch, AlignArgs);
+    uint32_t grid_plain, grid_rescue;
+    size_t align_smem;
+};
+
+static MapBatch with_work(const MapBatch& b, uint32_t* work_counter) {
+    MapBatch x = b;
+    x.work_counter = work_counter;
+    return x;
+}
+
+// Parameter tables (host libm, so scores are bit-identical to a CPU run) and the device copy of the parameters.
+static int map_params(gb_device* d, const gb_map_params* hp, uint32_t n_reads, bool paired, MapParamsDev& P) {
     int rc;
-    // ---- parameter tables (host libm, so scores are bit-identical to a CPU run) ----
     if (!d->tables_ready || d->tables_hard_hit_cap != hp->hard_hit_cap) {
         std::vector<double> hit(hp->hard_hit_cap + 1, 0.0);
         const double base_score = 1.0 + std::log((double)hp->hard_hit_cap);
@@ -247,7 +254,6 @@ int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const ui
         GB_CUDA(cudaStreamSynchronize(d->stream));
         d->tables_ready = true; d->tables_hard_hit_cap = hp->hard_hit_cap;
     }
-    MapParamsDev P;
     P.hit_cap = hp->hit_cap; P.hard_hit_cap = hp->hard_hit_cap; P.minimizer_score_fraction = hp->minimizer_score_fraction;
     P.minimizer_coverage_flank = hp->minimizer_coverage_flank; P.max_unique_min = hp->max_unique_min; P.num_bp_per_min = hp->num_bp_per_min;
     P.distance_limit = hp->distance_limit; P.min_extensions = hp->min_extensions; P.max_extensions = hp->max_extensions;
@@ -257,16 +263,229 @@ int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const ui
     P.extension_set_min_score = hp->extension_set_min_score; P.max_alignments = hp->max_alignments;
     P.max_extension_mismatches = hp->max_extension_mismatches; P.max_dozeu_cells = hp->max_dozeu_cells; P.do_dp = hp->do_dp;
     P.mapping_cap = hp->mapping_cap_per_read; P.edit_cap = hp->edit_cap_per_read;
-    P.max_multimaps = K; P.out_stride = n_reads;
+    P.max_multimaps = hp->max_multimaps; P.out_stride = n_reads;
     P.log_base = recover_log_base(d->sc);
     P.max_rescue_attempts = paired ? hp->max_rescue_attempts : 0; P.rescue_seed_limit = hp->rescue_seed_limit;
     P.paired_rescue_score_limit = hp->paired_rescue_score_limit; P.rescue_subgraph_stdevs = hp->rescue_subgraph_stdevs;
     P.rescue_likelihood_limit = hp->rescue_likelihood_limit;
     P.hit_score_table = d->t_hit.ptr; P.prob_at_least_one = d->t_plo.ptr; P.phred_prob = d->t_phred.ptr;
+    return GB_OK;
+}
+
+// K1: a first pass with small shared tables (8 blocks per SM), then the units that did not fit (many minimizers or
+// clusters) once more at the maximum table sizes.
+static int map_seed(MapRun& r) {
+    gb_device* d = r.d;
+    int rc;
+    if ((rc = d->p_retry.reserve(r.n_units + 1))) return rc;
+    for (int pass = 0; pass < 2; pass++) {
+        MapBatch bp = r.b;
+        bp.Mc = pass == 0 ? d->seed_mc : MAX_MINIMIZERS; bp.Cc = pass == 0 ? d->seed_cc : MAX_CLUSTERS;
+        bp.work_counter = pass == 0 ? &r.cur->seed_work : &r.cur->seed_retry_work;
+        bp.in_list = pass == 0 ? nullptr : d->p_retry.ptr; bp.in_count = pass == 0 ? nullptr : &r.cur->seed_retry_count;
+        bp.retry_list = d->p_retry.ptr; bp.retry_count = pass == 0 ? &r.cur->seed_retry_count : &r.cur->seed_retry_again;
+        // the cluster phases carve their scratch from the arrays that are dead after phase A
+        while (seed_dead_bytes(r.Lc, bp.Mc) < cluster_scratch_bytes(bp.Cc) && bp.Mc < MAX_MINIMIZERS) bp.Mc += 8;
+        uint32_t warps = SEED_WARPS;
+        while (warps > 1 && seed_smem_bytes(r.Lc, bp.Mc, bp.Cc) * warps > 200 * 1024) warps >>= 1;
+        const size_t smem = seed_smem_bytes(r.Lc, bp.Mc, bp.Cc) * warps;
+        const bool fixed_layout = r.Lc == 160 && bp.Mc == 64 && bp.Cc == 16;
+        auto seed_pe = fixed_layout ? seed_kernel_pe<160, 64, 16> : seed_kernel_pe<0, 0, 0>;
+        const void* kern = r.paired ? (const void*)seed_pe : (const void*)seed_kernel;
+        if (smem > 48 * 1024) GB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int bps = 0;
+        GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kern, warps * 32, smem));
+        if (bps < 1) bps = 1;
+        uint32_t grid = std::min<uint32_t>((uint32_t)(d->n_sms * bps), (r.n_units + warps - 1) / warps);
+        if (grid == 0) grid = 1;
+        if (r.paired) seed_pe<<<grid, warps * 32, smem, d->stream>>>(d->ix, r.P, bp, r.pools, PairBatch{d->p_pairs.ptr, r.fragment_limit});
+        else seed_kernel<<<grid, warps * 32, smem, d->stream>>>(d->ix, r.P, bp, r.pools);
+        d->launches++;
+        GB_CUDA(cudaGetLastError());
+        if ((rc = d->kt_mark(pass == 0 ? (r.paired ? "seed_kernel_pe" : "seed_kernel") : "seed_kernel(retry tables)"))) return rc;
+    }
+    return GB_OK;
+}
+
+// K2: extension over the items produced on the device.
+static int map_extend(MapRun& r) {
+    gb_device* d = r.d;
+    const size_t item_cap = r.item_cap;
+    const uint32_t max_ext = 48, path_cap = 384, mism_cap = 192;
+    int rc;
+    if ((rc = d->p_ext_count.reserve(item_cap))) return rc;
+    if ((rc = d->p_ext_status.reserve(item_cap))) return rc;
+    if ((rc = d->p_ext.reserve(item_cap * max_ext))) return rc;
+    if ((rc = d->p_path.reserve(item_cap * path_cap))) return rc;
+    if ((rc = d->p_mism.reserve(item_cap * mism_cap))) return rc;
+    // clusters whose seeds yield more extensions than those strides hold (repeats: a hundred seeds in one cluster, one
+    // extension per seed before GaplessExtender::extend removes duplicates) are redone with large strides
+    ExtendBig big;
+    big.cap = r.n_reads / 128 + 256; big.max_ext = 512; big.path_cap = 512 * 24; big.mism_cap = 512 * 4;
+    if ((rc = d->p_big_list.reserve(big.cap)) || (rc = d->p_big_of.reserve(item_cap)) || (rc = d->p_big_ext.reserve((size_t)big.cap * big.max_ext)) ||
+        (rc = d->p_big_path.reserve((size_t)big.cap * big.path_cap)) || (rc = d->p_big_mism.reserve((size_t)big.cap * big.mism_cap))) return rc;
+    GB_CUDA(cudaMemsetAsync(d->p_big_of.ptr, 0xff, sizeof(uint32_t) * item_cap, d->stream));
+    big.list = d->p_big_list.ptr; big.count = &r.cur->big_ext_count; big.big_of = d->p_big_of.ptr;
+    big.ext = d->p_big_ext.ptr; big.path = d->p_big_path.ptr; big.mism = d->p_big_mism.ptr;
+    ExtendParams ep;
+    ep.sc = d->sc; ep.max_mismatches = r.hp->max_extension_mismatches; ep.overlap_threshold = 0.8; ep.overlap_threshold_unused = 0.f;
+    ep.trim = 1; ep.max_ext = max_ext; ep.path_cap = path_cap; ep.mism_cap = mism_cap;
+    if ((rc = launch_extend_device(d, ep, r.b.reads, r.b.read_off, nullptr, d->p_ext_seeds.ptr, nullptr, d->p_items.ptr, &r.cur->item_cursor,
+                                   (uint32_t)item_cap, d->p_ext_count.ptr, d->p_ext_status.ptr, d->p_ext.ptr, d->p_path.ptr,
+                                   d->p_mism.ptr, r.Lc, &big))) return rc;
+    ExtView& ev = r.a.ev;
+    ev.ext_count = d->p_ext_count.ptr; ev.ext_status = d->p_ext_status.ptr; ev.ext = d->p_ext.ptr;
+    ev.path_pool = d->p_path.ptr; ev.mism_pool = d->p_mism.ptr; ev.max_ext = max_ext; ev.path_cap = path_cap; ev.mism_cap = mism_cap;
+    ev.big_of = d->p_big_of.ptr; ev.big_ext = d->p_big_ext.ptr; ev.big_path = d->p_big_path.ptr; ev.big_mism = d->p_big_mism.ptr;
+    ev.big_max_ext = big.max_ext; ev.big_path_cap = big.path_cap; ev.big_mism_cap = big.mism_cap;
+    return GB_OK;
+}
+
+// K3 setup: the warp-per-unit kernels' builds, grids and shared memory, their per-warp workspaces, the AlignArgs.
+static int setup_align(MapRun& r) {
+    gb_device* d = r.d; const gb_map_params* hp = r.hp;
+    // the five temporary path buffers of a warp go to shared memory when they fit beside the DP columns
+    const size_t slot_bytes = (size_t)hp->mapping_cap_per_read * sizeof(gb_mapping) + (size_t)hp->edit_cap_per_read * 4;
+    const uint32_t tmp_bytes = N_TEMP_SLOTS * slot_bytes <= 12 * 1024 ? (uint32_t)(N_TEMP_SLOTS * slot_bytes) : 0u;
+    const size_t smem = align_smem_per_warp(r.Lc, r.paired ? 2 : 1, tmp_bytes) * ALIGN_WARPS;
+    r.align = r.paired ? align_kernel_pe<false> : align_kernel;
+    if (smem > 48 * 1024) {
+        GB_CUDA(cudaFuncSetAttribute(r.align, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if (r.rescue) GB_CUDA(cudaFuncSetAttribute(align_kernel_pe<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    int bps = 0, bps_rescue = 0;
+    if (r.rescue) GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps_rescue, align_kernel_pe<true>, ALIGN_WARPS * 32, smem));
+    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, r.align, ALIGN_WARPS * 32, smem));
+    bps = std::max(1, std::min(bps, 4));                  // 4 bounds the per-warp tail workspaces (about 2 MB each)
+    r.grid_plain = std::max<uint32_t>(1u, std::min<uint32_t>((uint32_t)(d->n_sms * bps), (r.n_reads + ALIGN_WARPS - 1) / ALIGN_WARPS));
+    bps_rescue = std::max(1, std::min(bps_rescue, 2));    // + the rescue workspaces (about 2 MB each)
+    r.grid_rescue = r.rescue ? std::min<uint32_t>((uint32_t)(d->n_sms * bps_rescue), r.grid_plain) : r.grid_plain;
+    r.align_smem = smem;
+    const size_t n_warps = (size_t)r.grid_plain * ALIGN_WARPS;
+    const uint32_t tb_cells = hp->max_dozeu_cells + hp->max_dozeu_cells / 4 + 4096;
+    const size_t ws_stride = tail_ws_bytes(r.Lc, tb_cells);
+    const size_t cand_stride = (((size_t)hp->mapping_cap_per_read * sizeof(gb_mapping) + (size_t)hp->edit_cap_per_read * 4) * (N_SLOTS + N_TEMP_SLOTS) + 255) & ~(size_t)255;
+    int rc;
+    if ((rc = d->ws_tail.reserve(ws_stride * n_warps))) return rc;
+    if ((rc = d->ws_cand.reserve(cand_stride * n_warps))) return rc;
+    AlignArgs& a = r.a;
+    a.tmp_bytes = tmp_bytes;
+    if (r.rescue) {
+        a.rescue_stride = (rescue_ws_bytes(r.Lc) + 255) & ~(size_t)255;
+        if ((rc = d->ws_rescue.reserve(a.rescue_stride * (size_t)r.grid_rescue * ALIGN_WARPS))) return rc;
+        if ((rc = d->p_rescue.reserve(r.n_reads / 2 + 1))) return rc;
+        a.rescue_base = d->ws_rescue.ptr;
+    }
+    a.items = d->p_items.ptr; a.minimizers = d->p_min.ptr;
+    a.ws_base = d->ws_tail.ptr; a.ws_stride = ws_stride; a.cand_base = d->ws_cand.ptr; a.cand_stride = cand_stride;
+    a.tb_cells = tb_cells;
+    a.pairs = r.paired ? d->p_pairs.ptr : nullptr; a.frag_mean = hp->fragment_mean; a.frag_sd = hp->fragment_stdev;
+    return d->p_slow.reserve(r.n_units + 1);
+}
+
+// Thread-per-unit fast path; whatever it cannot finish goes to the slow list of the warp-per-unit kernels.
+static int map_align_fast(MapRun& r) {
+    gb_device* d = r.d;
+    FastArgs fa; fa.slow_list = d->p_slow.ptr; fa.slow_count = &r.cur->slow_count;
+    const uint32_t fgrid = std::max<uint32_t>(1u, std::min<uint32_t>((r.n_units + 127) / 128, (uint32_t)d->n_sms * 16));
+    auto fast = r.paired ? align_fast_kernel_pe : align_fast_kernel;
+    fast<<<fgrid, 128, 0, d->stream>>>(d->ix, r.P, d->sc, with_work(r.b, &r.cur->align_work), r.a, fa);
+    d->launches++;
+    GB_CUDA(cudaGetLastError());
+    int rc;
+    if ((rc = d->kt_mark(r.paired ? "align_fast_kernel_pe" : "align_fast_kernel"))) return rc;
+    r.a.slow_list = d->p_slow.ptr; r.a.slow_count = &r.cur->slow_count;
+    return GB_OK;
+}
+
+// Tails of the slow units: the plan (forests -> tiles), then the DP of every tile in its own compact kernel.  Wave 0: the
+// tails that are always aligned; the decide pass cancels what the reference would skip; wave 1: the rest.
+static int map_tails(MapRun& r) {
+    gb_device* d = r.d; MapCursors* cur = r.cur;
+    const size_t tile_cap = (size_t)r.n_reads * 4 + 4096;
+    const size_t unit_cap = std::min<size_t>((size_t)r.n_reads * 128 + (1u << 20), 0xfffffff0u);
+    const size_t path_cap = std::min<size_t>(tile_cap * 32, 0xfffffff0u);
+    int rc;
+    if ((rc = d->pl_entries.reserve((size_t)r.n_units * PLAN_PER_UNIT)) || (rc = d->pl_unit_base.reserve(r.n_units)) || (rc = d->pl_unit_count.reserve(r.n_units)) ||
+        (rc = d->pl_tiles.reserve(unit_cap * 16)) || (rc = d->pl_tile_off.reserve(tile_cap)) || (rc = d->pl_results.reserve(tile_cap)) ||
+        (rc = d->pl_lists.reserve(2 * TILE_CLASSES * tile_cap)) || (rc = d->pl_paths.reserve(path_cap)) || (rc = d->pl_stats.reserve(4))) return rc;
+    GB_CUDA(cudaMemsetAsync(d->pl_stats.ptr, 0, 4 * sizeof(uint64_t), d->stream));
+    PlanPools pp;
+    pp.entries = d->pl_entries.ptr; pp.unit_base = d->pl_unit_base.ptr; pp.unit_count = d->pl_unit_count.ptr;
+    pp.tiles = d->pl_tiles.ptr; pp.tile_units_cap = (uint32_t)unit_cap; pp.tile_units_cursor = &cur->tile_units;
+    pp.tile_off = d->pl_tile_off.ptr; pp.tile_cap = (uint32_t)tile_cap; pp.tile_cursor = &cur->tile_count;
+    pp.results = d->pl_results.ptr;
+    for (int c = 0; c < 2 * TILE_CLASSES; c++) pp.lists[c] = d->pl_lists.ptr + (size_t)c * tile_cap;
+    pp.list_count = cur->tile_list_count; pp.stats = d->pl_stats.ptr;
+    auto wave = [&](int w) {
+        return launch_tile_kernels(d, d->pl_tiles.ptr, d->pl_tile_off.ptr, d->pl_lists.ptr + (size_t)w * TILE_CLASSES * tile_cap, tile_cap,
+                                   cur->tile_list_count + w * TILE_CLASSES, cur->tile_work + w * TILE_CLASSES, d->pl_results.ptr,
+                                   d->pl_paths.ptr, (uint32_t)path_cap, &cur->tile_path_words);
+    };
+    auto plan = r.paired ? tail_plan_kernel<true> : tail_plan_kernel<false>;
+    plan<<<r.grid_plain, ALIGN_WARPS * 32, 0, d->stream>>>(d->ix, r.P, d->sc, with_work(r.b, &cur->plan_work), r.a, pp);
+    d->launches++;
+    GB_CUDA(cudaGetLastError());
+    if ((rc = d->kt_mark("tail_plan_kernel")) || (rc = wave(0))) return rc;
+    auto decide = r.paired ? tail_decide_kernel<true> : tail_decide_kernel<false>;
+    decide<<<r.grid_plain, ALIGN_WARPS * 32, 0, d->stream>>>(d->ix, r.P, d->sc, with_work(r.b, &cur->decide_work), r.a, pp);
+    d->launches++;
+    GB_CUDA(cudaGetLastError());
+    if ((rc = d->kt_mark("tail_decide_kernel")) || (rc = wave(1))) return rc;
+    PlanView& pv = r.a.plan;
+    pv.entries = d->pl_entries.ptr; pv.unit_base = d->pl_unit_base.ptr; pv.unit_count = d->pl_unit_count.ptr;
+    pv.tile_off = d->pl_tile_off.ptr; pv.results = d->pl_results.ptr; pv.path_pool = d->pl_paths.ptr; pv.stats = d->pl_stats.ptr;
+    return GB_OK;
+}
+
+// The warp-per-unit align kernel over the slow list.  Paired with rescue enabled, it defers the pairs that turn out to
+// have unpaired alignments to a second list, which the (larger, lower-occupancy) rescue build then redoes.
+static int map_align_warp(MapRun& r) {
+    gb_device* d = r.d; MapCursors* cur = r.cur;
+    if (r.paired) { r.a.rescue_list = d->p_rescue.ptr; r.a.rescue_count = &cur->rescue_count; }
+    r.align<<<r.grid_plain, ALIGN_WARPS * 32, r.align_smem, d->stream>>>(d->ix, r.P, d->sc, with_work(r.b, &cur->align_work), r.a);
+    d->launches++;
+    GB_CUDA(cudaGetLastError());
+    if (!r.rescue) return d->kt_mark(r.paired ? "align_kernel_pe" : "align_kernel");
+    int rc;
+    if ((rc = d->kt_mark("align_kernel_pe"))) return rc;
+    AlignArgs a = r.a;
+    a.slow_list = d->p_rescue.ptr; a.slow_count = &cur->rescue_count;
+    align_kernel_pe<true><<<r.grid_rescue, ALIGN_WARPS * 32, r.align_smem, d->stream>>>(d->ix, r.P, d->sc, with_work(r.b, &cur->rescue_work), a);
+    d->launches++;
+    GB_CUDA(cudaGetLastError());
+    return d->kt_mark("align_kernel_pe<rescue>");
+}
+
+// Device-resident mapping of a batch whose reads are already in HBM.
+int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
+               const uint64_t* d_read_off, uint32_t max_len, uint64_t total_bases,
+               gb_alignment* d_aln, uint8_t* d_status, bool paired,
+               gb_mapping* out_maps, uint64_t out_map_cap, uint32_t* out_edits, uint64_t out_edit_cap,
+               const uint64_t* d_run_base, uint32_t read_base, uint64_t* d_totals, uint32_t* d_overflow) {
+    int rc;
+    if (hp->max_multimaps == 0 || hp->max_multimaps > GB_MAX_MULTIMAPS) { g_last_error = "max_multimaps must be 1 .. GB_MAX_MULTIMAPS"; return GB_ERR_ARG; }
+    // the seeding kernels pack (node id << 10 | offset) into 32 bits (DevSeed.id_off): node ids stop at 2^22 - 1
+    if (d->ix.n_nodes > (1u << 23)) { g_last_error = "the mapping kernels address node ids below 2^22 (4 194 303); split the graph (the stage seams have no such limit)"; return GB_ERR_CAPACITY; }
+    const uint32_t K = hp->max_multimaps;            // records per read, rank-major: record j * n_reads + read
+    if ((uint64_t)n_reads * K * std::max(hp->mapping_cap_per_read, hp->edit_cap_per_read) > 0xffffffffull) { g_last_error = "chunk too large for 32-bit record offsets (reads x max_multimaps x cap)"; return GB_ERR_ARG; }
+    if ((rc = d->pad_maps.reserve((size_t)n_reads * K * hp->mapping_cap_per_read))) return rc;
+    if ((rc = d->pad_edits.reserve((size_t)n_reads * K * hp->edit_cap_per_read))) return rc;
+    if (paired) {
+        if (n_reads % 2 != 0) { g_last_error = "paired mapping needs an even number of reads"; return GB_ERR_ARG; }
+        if (hp->max_rescue_attempts != 0 && hp->rescue_seed_limit >= RESCUE_SEEDS) { g_last_error = "rescue_seed_limit must be below 128"; return GB_ERR_ARG; }
+        if (!(hp->fragment_stdev > 0)) { g_last_error = "paired mapping needs a forced fragment length distribution"; return GB_ERR_ARG; }
+    }
+    const uint32_t Lc = std::max<uint32_t>(32u, (max_len + 15u) & ~15u);
+    if (Lc > 512) { g_last_error = "reads longer than 512 bp are not supported by the short-read path"; return GB_ERR_ARG; }
+    MapRun r{};
+    r.d = d; r.hp = hp; r.n_reads = n_reads; r.n_units = paired ? n_reads / 2 : n_reads; r.K = K; r.Lc = Lc;
+    r.paired = paired; r.rescue = paired && hp->max_rescue_attempts != 0;
+    if ((rc = map_params(d, hp, n_reads, paired, r.P))) return rc;
 
     // ---- pools ----
     // Sized from per-read averages (48 minimizers, 64 seeds, 3 kept clusters) times d->pool_scale.  A chunk that needs
-    // more sets the sticky overflow word (cursor 13); the host-buffer entry points then double the scale and rerun the
+    // more sets the sticky MapCursors::pool_overflow; the host-buffer entry points then double the scale and rerun the
     // chunk (map_batch_host), gb_map_batch_device reports it through gb_device_pool_overflow.  Capacities stay below
     // 2^32 records (the cursors are 32-bit; pool_claim never lets one wrap).
     const double ps = d->pool_scale;
@@ -277,236 +496,55 @@ int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const ui
     if ((rc = d->p_seeds.reserve(seed_cap))) return rc;
     if ((rc = d->p_items.reserve(item_cap))) return rc;
     if ((rc = d->p_ext_seeds.reserve(ext_cap))) return rc;
-    if ((rc = d->p_cursors.reserve(48))) return rc;
-    GB_CUDA(cudaMemsetAsync(d->p_cursors.ptr, 0, 48 * sizeof(uint32_t), d->stream));
-    // 0 seed work, 1 min, 2 seed, 3 item, 4 ext, 5 extend work, 6 align work, 7 slow count, 8-10 seeding retry, 11-12 rescue, 13 pool overflow,
-    // 14 plan work, 15 big extension items, 16 tiles, 17 tile bytes / 16, 18-29 tile list counts (2 waves x 6 classes),
-    // 30 result path words, 31 decide work, 32-43 tile work
-    uint32_t* cur = d->p_cursors.ptr;
+    if ((rc = d->p_cursors.reserve(1))) return rc;
+    GB_CUDA(cudaMemsetAsync(d->p_cursors.ptr, 0, sizeof(MapCursors), d->stream));
+    MapCursors* cur = r.cur = d->p_cursors.ptr;
+    r.item_cap = item_cap;
     d->kt_reset();
     if (K > 1) {
         init_absent_kernel<<<d->n_sms * 4, 256, 0, d->stream>>>(d_aln, n_reads, n_reads * K, hp->mapping_cap_per_read, hp->edit_cap_per_read);
         d->launches++;
         GB_CUDA(cudaGetLastError());
     }
-
-    int32_t fragment_limit = 0;
     if (paired) {
         // rightward working copy of the reads (mate 2 reverse-complemented), :1503-1506
-        int rcw;
-        if ((rcw = d->w_reads.reserve(total_bases ? total_bases : 1))) return rcw;
-        if (d_quals) { if ((rcw = d->w_quals.reserve(total_bases ? total_bases : 1))) return rcw; }
+        if ((rc = d->w_reads.reserve(total_bases ? total_bases : 1))) return rc;
+        if (d_quals) { if ((rc = d->w_quals.reserve(total_bases ? total_bases : 1))) return rc; }
         prep_pairs_kernel<<<d->n_sms * 8, 256, 0, d->stream>>>(d_reads, d_quals, d_read_off, n_reads, d->w_reads.ptr, d_quals ? d->w_quals.ptr : nullptr);
         d->launches++;
         GB_CUDA(cudaGetLastError());
         d_reads = d->w_reads.ptr; if (d_quals) d_quals = d->w_quals.ptr;
-        fragment_limit = (int32_t)(int64_t)(hp->fragment_mean + hp->paired_distance_stdevs * hp->fragment_stdev);   // :1470
+        r.fragment_limit = (int32_t)(int64_t)(hp->fragment_mean + hp->paired_distance_stdevs * hp->fragment_stdev);   // :1470
         const uint32_t read_limit = std::max<uint32_t>(hp->distance_limit, max_len + 50);
-        if (fragment_limit < (int32_t)read_limit) { g_last_error = "fragment distance limit smaller than the read distance limit (the reference falls back to single-end, :1471)"; return GB_ERR_ARG; }
-        if ((rcw = d->p_pairs.reserve(n_reads / 2))) return rcw;
+        if (r.fragment_limit < (int32_t)read_limit) { g_last_error = "fragment distance limit smaller than the read distance limit (the reference falls back to single-end, :1471)"; return GB_ERR_ARG; }
+        if ((rc = d->p_pairs.reserve(n_reads / 2))) return rc;
     }
-    MapBatch b; b.reads = d_reads; b.quals = d_quals; b.read_off = d_read_off; b.n_reads = n_reads;
-    b.states = d->p_states.ptr; b.work_counter = cur + 0; b.Lc = Lc;
+    MapBatch& b = r.b;
+    b.reads = d_reads; b.quals = d_quals; b.read_off = d_read_off; b.n_reads = n_reads;
+    b.states = d->p_states.ptr; b.work_counter = &cur->seed_work; b.Lc = Lc;
     b.in_list = nullptr; b.in_count = nullptr; b.retry_list = nullptr; b.retry_count = nullptr; b.Mc = MAX_MINIMIZERS; b.Cc = MAX_CLUSTERS; b.Ns = d->seed_ns;
-    SeedPools pools;
-    pools.dbg_clusters = d->dbg_clusters; pools.overflow = cur + 13;
-    pools.minimizers = d->p_min.ptr; pools.min_cap = (uint32_t)min_cap; pools.min_cursor = cur + 1;
-    pools.seeds = d->p_seeds.ptr; pools.seed_cap = (uint32_t)seed_cap; pools.seed_cursor = cur + 2;
-    pools.items = d->p_items.ptr; pools.item_cap = (uint32_t)item_cap; pools.item_cursor = cur + 3;
-    pools.ext_seeds = d->p_ext_seeds.ptr; pools.ext_cap = (uint32_t)ext_cap; pools.ext_cursor = cur + 4;
+    SeedPools& pools = r.pools;
+    pools.dbg_clusters = d->dbg_clusters; pools.overflow = &cur->pool_overflow;
+    pools.minimizers = d->p_min.ptr; pools.min_cap = (uint32_t)min_cap; pools.min_cursor = &cur->min_cursor;
+    pools.seeds = d->p_seeds.ptr; pools.seed_cap = (uint32_t)seed_cap; pools.seed_cursor = &cur->seed_cursor;
+    pools.items = d->p_items.ptr; pools.item_cap = (uint32_t)item_cap; pools.item_cursor = &cur->item_cursor;
+    pools.ext_seeds = d->p_ext_seeds.ptr; pools.ext_cap = (uint32_t)ext_cap; pools.ext_cursor = &cur->ext_cursor;
+    r.a.aln = d_aln; r.a.maps = d->pad_maps.ptr; r.a.edits = d->pad_edits.ptr; r.a.status = d_status;
 
     GB_CUDA(cudaEventRecord(d->ev_stage[0], d->stream));
-    if ((rc = d->kt_mark("start"))) return rc;
-    // ---- K1: a first pass with small shared tables (8 blocks per SM), then the units that did not
-    // fit (many minimizers or clusters) once more at the maximum table sizes ----
-    {
-        const uint32_t n_units = paired ? n_reads / 2 : n_reads;
-        if ((rc = d->p_retry.reserve(n_units + 1))) return rc;
-        for (int pass = 0; pass < 2; pass++) {
-            MapBatch bp = b;
-            bp.Mc = pass == 0 ? d->seed_mc : MAX_MINIMIZERS; bp.Cc = pass == 0 ? d->seed_cc : MAX_CLUSTERS;
-            bp.work_counter = pass == 0 ? cur + 0 : cur + 9;
-            bp.in_list = pass == 0 ? nullptr : d->p_retry.ptr; bp.in_count = pass == 0 ? nullptr : cur + 8;
-            bp.retry_list = d->p_retry.ptr; bp.retry_count = pass == 0 ? cur + 8 : cur + 10;
-            // the cluster phases carve their scratch from the arrays that are dead after phase A
-            while (seed_dead_bytes(Lc, bp.Mc) < cluster_scratch_bytes(bp.Cc) && bp.Mc < MAX_MINIMIZERS) bp.Mc += 8;
-            uint32_t warps = SEED_WARPS;
-            while (warps > 1 && seed_smem_bytes(Lc, bp.Mc, bp.Cc) * warps > 200 * 1024) warps >>= 1;
-            const size_t smem = seed_smem_bytes(Lc, bp.Mc, bp.Cc) * warps;
-            const bool fixed_layout = paired && Lc == 160 && bp.Mc == 64 && bp.Cc == 16;
-            if (smem > 48 * 1024) {
-                GB_CUDA(cudaFuncSetAttribute(seed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                GB_CUDA(cudaFuncSetAttribute(seed_kernel_pe<0, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                GB_CUDA(cudaFuncSetAttribute(seed_kernel_pe<160, 64, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            }
-            int bps = 0;
-            if (paired && fixed_layout) GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, seed_kernel_pe<160, 64, 16>, warps * 32, smem));
-            else if (paired) GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, seed_kernel_pe<0, 0, 0>, warps * 32, smem));
-            else GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, seed_kernel, warps * 32, smem));
-            if (bps < 1) bps = 1;
-            uint32_t grid = std::min<uint32_t>((uint32_t)(d->n_sms * bps), (n_units + warps - 1) / warps);
-            if (grid == 0) grid = 1;
-            if (paired) { PairBatch pbatch; pbatch.pairs = d->p_pairs.ptr; pbatch.fragment_limit = fragment_limit;
-                          if (fixed_layout) seed_kernel_pe<160, 64, 16><<<grid, warps * 32, smem, d->stream>>>(d->ix, P, bp, pools, pbatch);
-                          else seed_kernel_pe<0, 0, 0><<<grid, warps * 32, smem, d->stream>>>(d->ix, P, bp, pools, pbatch); }
-            else seed_kernel<<<grid, warps * 32, smem, d->stream>>>(d->ix, P, bp, pools);
-            d->launches++;
-            GB_CUDA(cudaGetLastError());
-            if ((rc = d->kt_mark(pass == 0 ? (paired ? "seed_kernel_pe" : "seed_kernel") : "seed_kernel(retry tables)"))) return rc;
-        }
-    }
+    if ((rc = d->kt_mark("start")) || (rc = map_seed(r))) return rc;
     GB_CUDA(cudaEventRecord(d->ev_stage[1], d->stream));
     if (d->debug_stop_after_seed) return GB_OK;              // gb_debug_seed_stage reads the pools as the seeding kernels left them
-    // ---- K2: extension over the items produced on the device ----
-    const uint32_t max_ext = 48, path_cap = 384, mism_cap = 192;
-    if ((rc = d->p_ext_count.reserve(item_cap))) return rc;
-    if ((rc = d->p_ext_status.reserve(item_cap))) return rc;
-    if ((rc = d->p_ext.reserve(item_cap * max_ext))) return rc;
-    if ((rc = d->p_path.reserve(item_cap * path_cap))) return rc;
-    if ((rc = d->p_mism.reserve(item_cap * mism_cap))) return rc;
-    // clusters whose seeds yield more extensions than those strides hold (repeats: a hundred seeds in one cluster, one
-    // extension per seed before GaplessExtender::extend removes duplicates) are redone with large strides
-    ExtendBig big;
-    big.cap = n_reads / 128 + 256; big.max_ext = 512; big.path_cap = 512 * 24; big.mism_cap = 512 * 4;
-    if ((rc = d->p_big_list.reserve(big.cap)) || (rc = d->p_big_of.reserve(item_cap)) || (rc = d->p_big_ext.reserve((size_t)big.cap * big.max_ext)) ||
-        (rc = d->p_big_path.reserve((size_t)big.cap * big.path_cap)) || (rc = d->p_big_mism.reserve((size_t)big.cap * big.mism_cap))) return rc;
-    GB_CUDA(cudaMemsetAsync(d->p_big_of.ptr, 0xff, sizeof(uint32_t) * item_cap, d->stream));
-    big.list = d->p_big_list.ptr; big.count = cur + 15; big.big_of = d->p_big_of.ptr;
-    big.ext = d->p_big_ext.ptr; big.path = d->p_big_path.ptr; big.mism = d->p_big_mism.ptr;
-    {
-        ExtendParams ep;
-        ep.sc = d->sc; ep.max_mismatches = hp->max_extension_mismatches; ep.overlap_threshold = 0.8; ep.overlap_threshold_unused = 0.f;
-        ep.trim = 1; ep.max_ext = max_ext; ep.path_cap = path_cap; ep.mism_cap = mism_cap;
-        if ((rc = launch_extend_device(d, ep, d_reads, d_read_off, nullptr, d->p_ext_seeds.ptr, nullptr, d->p_items.ptr, cur + 3,
-                                       (uint32_t)item_cap, d->p_ext_count.ptr, d->p_ext_status.ptr, d->p_ext.ptr, d->p_path.ptr,
-                                       d->p_mism.ptr, Lc, &big))) return rc;
-    }
+    if ((rc = map_extend(r))) return rc;
     GB_CUDA(cudaEventRecord(d->ev_stage[2], d->stream));
-    // ---- K3 ----
-    {
-        const uint32_t W = Lc + 1;
-        // the five temporary path buffers of a warp go to shared memory when they fit beside the DP columns
-        const size_t slot_bytes = (size_t)hp->mapping_cap_per_read * sizeof(gb_mapping) + (size_t)hp->edit_cap_per_read * 4;
-        const uint32_t tmp_bytes = N_TEMP_SLOTS * slot_bytes <= 12 * 1024 ? (uint32_t)(N_TEMP_SLOTS * slot_bytes) : 0u;
-        const size_t per_warp = (((size_t)Lc * (paired ? 5 : 3) + 15) & ~(size_t)15) + (size_t)W * 4 * 4 + 64 + tmp_bytes;
-        const size_t smem = per_warp * ALIGN_WARPS;
-        if (smem > 48 * 1024) {
-            GB_CUDA(cudaFuncSetAttribute(align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            GB_CUDA(cudaFuncSetAttribute(align_kernel_pe<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            GB_CUDA(cudaFuncSetAttribute(align_kernel_pe<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        }
-        int bps = 0;
-        const bool rescue = paired && hp->max_rescue_attempts != 0;
-        int bps_rescue = 0;
-        if (rescue) GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps_rescue, align_kernel_pe<true>, ALIGN_WARPS * 32, smem));
-        if (paired) GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, align_kernel_pe<false>, ALIGN_WARPS * 32, smem));
-        else GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, align_kernel, ALIGN_WARPS * 32, smem));
-        if (bps < 1) bps = 1;
-        if (bps > 4) bps = 4;          // bounds the per-warp tail workspaces (about 2 MB each)
-        uint32_t grid_plain = std::min<uint32_t>((uint32_t)(d->n_sms * bps), (n_reads + ALIGN_WARPS - 1) / ALIGN_WARPS);
-        if (grid_plain == 0) grid_plain = 1;
-        bps_rescue = std::max(1, std::min(bps_rescue, 2));     // + the rescue workspaces (about 2 MB each)
-        uint32_t grid = rescue ? std::min<uint32_t>((uint32_t)(d->n_sms * bps_rescue), grid_plain) : grid_plain;
-        const size_t n_warps = (size_t)grid_plain * ALIGN_WARPS;
-        const uint32_t tb_cells = hp->max_dozeu_cells + hp->max_dozeu_cells / 4 + 4096;
-        const size_t ws_stride = tail_ws_bytes(Lc, tb_cells);
-        const size_t cand_stride = (((size_t)hp->mapping_cap_per_read * sizeof(gb_mapping) + (size_t)hp->edit_cap_per_read * 4) * (N_SLOTS + N_TEMP_SLOTS) + 255) & ~(size_t)255;
-        if ((rc = d->ws_tail.reserve(ws_stride * n_warps))) return rc;
-        if ((rc = d->ws_cand.reserve(cand_stride * n_warps))) return rc;
-        AlignArgs a;
-        a.plan.entries = nullptr; a.plan.unit_base = nullptr; a.plan.unit_count = nullptr; a.plan.tile_off = nullptr; a.plan.results = nullptr; a.plan.path_pool = nullptr; a.plan.stats = nullptr;
-        a.rescue_base = nullptr; a.rescue_stride = 0; a.tmp_bytes = tmp_bytes;
-        if (rescue) {
-            a.rescue_stride = (rescue_ws_bytes(Lc) + 255) & ~(size_t)255;
-            if ((rc = d->ws_rescue.reserve(a.rescue_stride * (size_t)grid * ALIGN_WARPS))) return rc;
-            if ((rc = d->p_rescue.reserve(n_reads / 2 + 1))) return rc;
-            a.rescue_base = d->ws_rescue.ptr;
-        }
-        a.items = d->p_items.ptr; a.minimizers = d->p_min.ptr;
-        a.ev.ext_count = d->p_ext_count.ptr; a.ev.ext_status = d->p_ext_status.ptr; a.ev.ext = d->p_ext.ptr;
-        a.ev.path_pool = d->p_path.ptr; a.ev.mism_pool = d->p_mism.ptr; a.ev.max_ext = max_ext; a.ev.path_cap = path_cap; a.ev.mism_cap = mism_cap;
-        a.ev.big_of = d->p_big_of.ptr; a.ev.big_ext = d->p_big_ext.ptr; a.ev.big_path = d->p_big_path.ptr; a.ev.big_mism = d->p_big_mism.ptr;
-        a.ev.big_max_ext = big.max_ext; a.ev.big_path_cap = big.path_cap; a.ev.big_mism_cap = big.mism_cap;
-        a.ws_base = d->ws_tail.ptr; a.ws_stride = ws_stride; a.cand_base = d->ws_cand.ptr; a.cand_stride = cand_stride;
-        a.aln = d_aln; a.maps = d_maps; a.edits = d_edits; a.status = d_status; a.tb_cells = tb_cells;
-        a.pairs = paired ? d->p_pairs.ptr : nullptr; a.frag_mean = hp->fragment_mean; a.frag_sd = hp->fragment_stdev;
-        MapBatch b3 = b; b3.work_counter = cur + 6;
-        // thread-per-unit fast path first; whatever it cannot finish goes to the warp-per-unit kernel
-        const uint32_t n_units = paired ? n_reads / 2 : n_reads;
-        if ((rc = d->p_slow.reserve(n_units + 1))) return rc;
-        FastArgs fa; fa.slow_list = d->p_slow.ptr; fa.slow_count = cur + 7;
-        const uint32_t fgrid = std::max<uint32_t>(1u, std::min<uint32_t>((n_units + 127) / 128, (uint32_t)d->n_sms * 16));
-        a.slow_list = nullptr; a.slow_count = nullptr;
-        if (paired) {
-            if (d->fast_minb == 12) align_fast_kernel_pe<12><<<fgrid, 128, 0, d->stream>>>(d->ix, P, d->sc, b3, a, fa);
-            else if (d->fast_minb == 16) align_fast_kernel_pe<16><<<fgrid, 128, 0, d->stream>>>(d->ix, P, d->sc, b3, a, fa);
-            else align_fast_kernel_pe<0><<<fgrid, 128, 0, d->stream>>>(d->ix, P, d->sc, b3, a, fa);
-        }
-        else align_fast_kernel<<<fgrid, 128, 0, d->stream>>>(d->ix, P, d->sc, b3, a, fa);
-        d->launches++;
-        GB_CUDA(cudaGetLastError());
-        if ((rc = d->kt_mark(paired ? "align_fast_kernel_pe" : "align_fast_kernel"))) return rc;
-        a.slow_list = d->p_slow.ptr; a.slow_count = cur + 7;
-        // ---- tails of the slow units: plan (forests -> tiles), then the DP of every tile in its own compact kernel ----
-        if (hp->do_dp && d->use_tiles) {
-            const size_t tile_cap = (size_t)n_reads * 4 + 4096;
-            const size_t unit_cap = std::min<size_t>((size_t)n_reads * 128 + (1u << 20), 0xfffffff0u);
-            const size_t path_cap = std::min<size_t>(tile_cap * 32, 0xfffffff0u);
-            if ((rc = d->pl_entries.reserve((size_t)n_units * PLAN_PER_UNIT)) || (rc = d->pl_unit_base.reserve(n_units)) || (rc = d->pl_unit_count.reserve(n_units)) ||
-                (rc = d->pl_tiles.reserve(unit_cap * 16)) || (rc = d->pl_tile_off.reserve(tile_cap)) || (rc = d->pl_results.reserve(tile_cap)) ||
-                (rc = d->pl_lists.reserve(2 * TILE_CLASSES * tile_cap)) || (rc = d->pl_paths.reserve(path_cap)) || (rc = d->pl_stats.reserve(4))) return rc;
-            GB_CUDA(cudaMemsetAsync(d->pl_stats.ptr, 0, 4 * sizeof(uint64_t), d->stream));
-            PlanPools pp;
-            pp.entries = d->pl_entries.ptr; pp.unit_base = d->pl_unit_base.ptr; pp.unit_count = d->pl_unit_count.ptr;
-            pp.tiles = d->pl_tiles.ptr; pp.tile_units_cap = (uint32_t)unit_cap; pp.tile_units_cursor = cur + 17;
-            pp.tile_off = d->pl_tile_off.ptr; pp.tile_cap = (uint32_t)tile_cap; pp.tile_cursor = cur + 16;
-            pp.results = d->pl_results.ptr;
-            for (int c = 0; c < 2 * TILE_CLASSES; c++) pp.lists[c] = d->pl_lists.ptr + (size_t)c * tile_cap;
-            pp.list_count = cur + 18; pp.stats = d->pl_stats.ptr;
-            MapBatch bpl = b3; bpl.work_counter = cur + 14;
-            if (paired) tail_plan_kernel<true><<<grid_plain, ALIGN_WARPS * 32, 0, d->stream>>>(d->ix, P, d->sc, bpl, a, pp);
-            else tail_plan_kernel<false><<<grid_plain, ALIGN_WARPS * 32, 0, d->stream>>>(d->ix, P, d->sc, bpl, a, pp);
-            d->launches++;
-            GB_CUDA(cudaGetLastError());
-            if ((rc = d->kt_mark("tail_plan_kernel"))) return rc;
-            // wave 0: the tails that are always aligned; the decide pass cancels what the reference would skip; wave 1: the rest
-            if ((rc = launch_tile_kernels(d, d->pl_tiles.ptr, d->pl_tile_off.ptr, d->pl_lists.ptr, tile_cap, cur + 18, cur + 32, d->pl_results.ptr,
-                                          d->pl_paths.ptr, (uint32_t)path_cap, cur + 30))) return rc;
-            MapBatch bdc = b3; bdc.work_counter = cur + 31;
-            if (paired) tail_decide_kernel<true><<<grid_plain, ALIGN_WARPS * 32, 0, d->stream>>>(d->ix, P, d->sc, bdc, a, pp);
-            else tail_decide_kernel<false><<<grid_plain, ALIGN_WARPS * 32, 0, d->stream>>>(d->ix, P, d->sc, bdc, a, pp);
-            d->launches++;
-            GB_CUDA(cudaGetLastError());
-            if ((rc = d->kt_mark("tail_decide_kernel"))) return rc;
-            if ((rc = launch_tile_kernels(d, d->pl_tiles.ptr, d->pl_tile_off.ptr, d->pl_lists.ptr + (size_t)TILE_CLASSES * tile_cap, tile_cap, cur + 18 + TILE_CLASSES,
-                                          cur + 32 + TILE_CLASSES, d->pl_results.ptr, d->pl_paths.ptr, (uint32_t)path_cap, cur + 30))) return rc;
-            a.plan.entries = d->pl_entries.ptr; a.plan.unit_base = d->pl_unit_base.ptr; a.plan.unit_count = d->pl_unit_count.ptr;
-            a.plan.tile_off = d->pl_tile_off.ptr; a.plan.results = d->pl_results.ptr; a.plan.path_pool = d->pl_paths.ptr; a.plan.stats = d->pl_stats.ptr;
-        }
-        if (paired) {
-            // the plain kernel takes every listed pair; with rescue enabled it defers the pairs that turn out to have
-            // unpaired alignments to a second list, which the (larger, lower-occupancy) rescue instantiation redoes
-            a.rescue_list = d->p_rescue.ptr; a.rescue_count = cur + 11;
-            align_kernel_pe<false><<<grid_plain, ALIGN_WARPS * 32, smem, d->stream>>>(d->ix, P, d->sc, b3, a);
-            if (rescue) {
-                d->launches++;
-                GB_CUDA(cudaGetLastError());
-                if ((rc = d->kt_mark("align_kernel_pe"))) return rc;
-                b3.work_counter = cur + 12;
-                a.slow_list = d->p_rescue.ptr; a.slow_count = cur + 11;
-                align_kernel_pe<true><<<grid, ALIGN_WARPS * 32, smem, d->stream>>>(d->ix, P, d->sc, b3, a);
-            }
-        }
-        else align_kernel<<<grid, ALIGN_WARPS * 32, smem, d->stream>>>(d->ix, P, d->sc, b3, a);
-        d->launches++;
-        GB_CUDA(cudaGetLastError());
-        if ((rc = d->kt_mark(!paired ? "align_kernel" : (rescue ? "align_kernel_pe<rescue>" : "align_kernel_pe")))) return rc;
-    }
+    if ((rc = setup_align(r)) || (rc = map_align_fast(r))) return rc;
+    if (hp->do_dp && d->use_tiles && (rc = map_tails(r))) return rc;
+    if ((rc = map_align_warp(r))) return rc;
     GB_CUDA(cudaEventRecord(d->ev_stage[3], d->stream));
-    if ((rc = compact_outputs(d, n_reads * K, n_reads, d_aln, d_maps, d_edits, hp->mapping_cap_per_read, hp->edit_cap_per_read,
+    if ((rc = compact_outputs(d, n_reads * K, n_reads, d_aln, d->pad_maps.ptr, d->pad_edits.ptr, hp->mapping_cap_per_read, hp->edit_cap_per_read,
                               out_maps, out_map_cap, out_edits, out_edit_cap, d_run_base, read_base, d_totals, d_status))) return rc;
     if ((rc = d->kt_mark("compact (2 scans + gather)"))) return rc;
-    if (d_overflow) GB_CUDA(cudaMemcpyAsync(d_overflow, cur + 13, sizeof(uint32_t), cudaMemcpyDeviceToDevice, d->stream));
+    if (d_overflow) GB_CUDA(cudaMemcpyAsync(d_overflow, &cur->pool_overflow, sizeof(uint32_t), cudaMemcpyDeviceToDevice, d->stream));
     GB_CUDA(cudaEventRecord(d->ev_stage[4], d->stream));
     return GB_OK;
 }
@@ -691,7 +729,7 @@ extern "C" int gb_device_pool_overflow(gb_device* d, int* overflowed) {
     GB_CUDA(cudaSetDevice(d->device));
     GB_CUDA(cudaStreamSynchronize(d->stream));
     uint32_t flag = 0;
-    GB_CUDA(cudaMemcpy(&flag, d->p_cursors.ptr + 13, sizeof flag, cudaMemcpyDeviceToHost));
+    GB_CUDA(cudaMemcpy(&flag, &d->p_cursors.ptr->pool_overflow, sizeof flag, cudaMemcpyDeviceToHost));
     if (flag) { *overflowed = 1; if (d->pool_scale < 1024.0) d->pool_scale *= 2.0; d->pool_reruns++; }
     return GB_OK;
 }
@@ -716,7 +754,7 @@ extern "C" int gb_debug_seed_stage(gb_device* d, const gb_map_params* hp, int pa
             (rc = d_aln.reserve((size_t)n_reads * std::max<uint32_t>(hp->max_multimaps, 1u))) || (rc = d_dbg.reserve((size_t)n_reads * MAX_CLUSTERS))) return rc;
         GB_CUDA(cudaMemsetAsync(d_dbg.ptr, 0, sizeof(DbgCluster) * (size_t)n_reads * MAX_CLUSTERS, d->stream));
         std::vector<ReadState> st(n_reads);
-        uint32_t cursors[16];
+        MapCursors cursors;
         for (int attempt = 0;; attempt++) {
             d->dbg_clusters = d_dbg.ptr; d->debug_stop_after_seed = true;
             rc = map_device(d, hp, n_reads, d_reads.ptr, quals ? d_quals.ptr : nullptr, d_off.ptr, max_len, total, d_aln.ptr, d_status.ptr, paired != 0,
@@ -724,13 +762,14 @@ extern "C" int gb_debug_seed_stage(gb_device* d, const gb_map_params* hp, int pa
             d->dbg_clusters = nullptr; d->debug_stop_after_seed = false;
             if (rc) return rc;
             GB_CUDA(cudaStreamSynchronize(d->stream));
-            GB_CUDA(cudaMemcpy(cursors, d->p_cursors.ptr, sizeof cursors, cudaMemcpyDeviceToHost));
-            if (!cursors[13]) break;
+            GB_CUDA(cudaMemcpy(&cursors, d->p_cursors.ptr, sizeof cursors, cudaMemcpyDeviceToHost));
+            if (!cursors.pool_overflow) break;
             if (attempt >= 10) { g_last_error = "seed stage: pools overflow"; return GB_ERR_CAPACITY; }
             d->pool_scale *= 2.0; d->pool_reruns++;
         }
         GB_CUDA(cudaMemcpy(st.data(), d->p_states.ptr, sizeof(ReadState) * n_reads, cudaMemcpyDeviceToHost));
-        std::vector<DevMinimizer> hm(cursors[1]); std::vector<DevSeed> hs(cursors[2]); std::vector<DevItem> hi(cursors[3]); std::vector<gb_seed> he(cursors[4]);
+        std::vector<DevMinimizer> hm(cursors.min_cursor); std::vector<DevSeed> hs(cursors.seed_cursor); std::vector<DevItem> hi(cursors.item_cursor);
+        std::vector<gb_seed> he(cursors.ext_cursor);
         std::vector<DbgCluster> hc((size_t)n_reads * MAX_CLUSTERS);
         if (!hm.empty()) GB_CUDA(cudaMemcpy(hm.data(), d->p_min.ptr, sizeof(DevMinimizer) * hm.size(), cudaMemcpyDeviceToHost));
         if (!hs.empty()) GB_CUDA(cudaMemcpy(hs.data(), d->p_seeds.ptr, sizeof(DevSeed) * hs.size(), cudaMemcpyDeviceToHost));
@@ -837,199 +876,4 @@ extern "C" int gb_kernel_times(gb_device* d, uint32_t cap, char* names, float* m
         (*n_out)++;
     }
     return GB_OK;
-}
-
-// ---------------------------------------------------------------------------------------
-// B3 stage seam: Aligner::align_pinned(xdrop = true), batched over explicit haplotype trees
-// (aligner.cpp:628-686 -> DozeuInterface::align_pinned dozeu_interface.cpp:724-766).
-// ---------------------------------------------------------------------------------------
-namespace gb {
-
-struct XdropBatch {
-    const int32_t* tree_parent; const uint32_t* tree_node; const uint64_t* tree_off; const uint32_t* root_trim;
-    const uint8_t* query; const uint64_t* query_off; const uint32_t* max_gap;
-    uint32_t n; uint32_t Lc;
-    SeamOut out;
-    uint8_t* ws_base; size_t ws_stride; uint32_t tb_cells;
-    uint32_t* work_counter;
-    uint8_t* skip;                   // [n] 1: the problem ran on xdrop_tile_kernel instead
-};
-
-// results of the tile kernel -> the seam's output arrays.  A tile that outgrew the tile's own path capacities
-// (TILE_MAP_CAP / TILE_EDIT_CAP / TILE_STEP_CAP) gives its problem back to xdrop_kernel, which aligns it within the
-// caller's map_cap / edit_cap: the seam's answer does not depend on which kernel a problem was routed to.
-__global__ void unpack_tile_results_kernel(XdropBatch b, const TileResult* results, const uint32_t* path_pool) {
-    const uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (p >= b.n || !b.skip[p]) return;
-    const TileResult tr = results[p];
-    if (tr.status != GB_TILE_ST_OK) {
-        if (lane == 0) b.skip[p] = 0;
-        return;
-    }
-    uint32_t status = GB_ITEM_OK;
-    if (tr.n_maps > b.out.map_cap || tr.n_edits > b.out.edit_cap) status = GB_ITEM_OUT_FULL;
-    if (status == GB_ITEM_OK) {
-        const gb_mapping* gm = reinterpret_cast<const gb_mapping*>(path_pool + tr.path_off);
-        const uint32_t* ge = path_pool + tr.path_off + 2 * tr.n_maps;
-        for (uint32_t i = lane; i < tr.n_maps; i += 32) b.out.maps[(size_t)p * b.out.map_cap + i] = gm[i];
-        for (uint32_t i = lane; i < tr.n_edits; i += 32) b.out.edits[(size_t)p * b.out.edit_cap + i] = ge[i];
-    }
-    const bool ok = status == GB_ITEM_OK;
-    b.out.store(p, ok ? tr.score : 0, ok ? tr.n_maps : 0, ok ? tr.n_edits : 0, status);
-}
-
-__global__ void __launch_bounds__(ALIGN_WARPS * 32, 4)
-xdrop_kernel(DevIndex ix, DevScores sc, XdropBatch b) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t gwarp = blockIdx.x * ALIGN_WARPS + warp;
-    uint8_t* q;
-    const DpSmem dps = dp_smem_carve(smem, warp, b.Lc, q);
-    const TailWs ws = carve_tail_ws(b.ws_base + (size_t)gwarp * b.ws_stride, b.Lc, b.tb_cells);
-    while (true) {
-        uint32_t p = 0;
-        if (lane == 0) p = atomicAdd(b.work_counter, 1u);
-        p = __shfl_sync(FULL, p, 0);
-        if (p >= b.n) break;
-        if (b.skip && b.skip[p]) continue;
-        const uint64_t t_begin = b.tree_off[p]; const uint32_t nt = (uint32_t)(b.tree_off[p + 1] - t_begin);
-        const uint64_t q_begin = b.query_off[p]; const uint32_t m = (uint32_t)(b.query_off[p + 1] - q_begin);
-        uint32_t status = GB_ITEM_OK; int32_t score = 0;
-        PathBuf out = b.out.path(p);
-        if (nt == 0 || nt > TAIL_T_CAP || m > b.Lc) status = GB_ITEM_OUT_FULL;
-        else {
-            for (uint32_t i = lane; i < m; i += 32) q[i] = dp_query_base(b.query[q_begin + i]);
-            // materialise the tree (depths from parents)
-            if (lane == 0) {
-                for (uint32_t i = 0; i < nt; i++) {
-                    TreeNode t; t.parent = b.tree_parent[t_begin + i]; t.node = b.tree_node[t_begin + i];
-                    const gb_node_rec nr = load_node(ix, t.node);
-                    const uint32_t trim = t.parent < 0 ? b.root_trim[p] : 0u;
-                    t.seq_off = nr.seq_off + trim; t.len = nr.len - trim;
-                    t.depth = t.parent < 0 ? 0u : ws.tree[t.parent].depth + 1;
-                    t.tb_col = 0; t.lineage_max = 0; t.computed = 0;
-                    ws.tree[i] = t;
-                }
-            }
-            __syncwarp();
-            bool ovf = false;
-            score = xdrop_tree(ix, sc, ws, dps, 0, nt, q, m, max(b.max_gap[p], 1u), out, ovf);
-            if (ovf || out.overflow) status = GB_ITEM_OUT_FULL;
-        }
-        b.out.store(p, score, out.n_maps, out.n_edits, status);
-        __syncwarp();
-    }
-}
-
-} // namespace gb
-
-extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
-                                     const int32_t* tree_parent, const uint32_t* tree_node, const uint64_t* tree_off,
-                                     const uint32_t* root_trim, const uint8_t* query, const uint64_t* query_off,
-                                     const uint32_t* max_gap, uint32_t map_cap, uint32_t edit_cap,
-                                     int32_t* score, gb_mapping* maps, uint32_t* edits, uint32_t* n_maps, uint32_t* n_edits,
-                                     uint8_t* status) {
-    if (!d || !tree_parent || !tree_node || !tree_off || !root_trim || !query || !query_off || !max_gap || !score || !maps ||
-        !edits || !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
-    if (n == 0) return GB_OK;
-    // ---- validation, before anything reaches the device: known nodes; one root, first; the nodes in DFS visit order (both
-    // kernels keep one DP column per tree level, which a node's parent must still own); the root trim leaves a base; fewer
-    // than TAIL_D_CAP levels ----
-    std::vector<uint64_t> prob_bases(n, 0); std::vector<uint32_t> prob_depth(n, 0), lineage;
-    uint32_t max_q = 0, Lc;
-    auto fail = [](const char* what) { g_last_error = std::string("gb_xdrop_pinned_batch: ") + what; return GB_ERR_ARG; };
-    for (uint32_t i = 0; i < n; i++) {
-        max_q = std::max<uint32_t>(max_q, (uint32_t)(query_off[i + 1] - query_off[i]));
-        const uint64_t t0 = tree_off[i]; const uint32_t ntree = (uint32_t)(tree_off[i + 1] - t0);
-        if (ntree == 0) return fail("empty tree");
-        if (max_gap[i] > 65535) return fail("max_gap above 65535");      // vg's max_gap is a uint16_t
-        lineage.clear();                     // root .. previous node
-        for (uint32_t x = 0; x < ntree; x++) {
-            const uint32_t v = tree_node[t0 + x]; const int32_t par = tree_parent[t0 + x];
-            if (v < 2 || v >= d->ix.n_nodes || d->h_node_len[v] == 0) return fail("unknown node");
-            if (x == 0 && par >= 0) return fail("the first tree node is not a root");
-            if (x > 0 && par < 0) return fail("more than one root");
-            if (par >= (int32_t)x) return fail("a parent does not precede its child");
-            while (par >= 0 && !lineage.empty() && lineage.back() != (uint32_t)par) lineage.pop_back();
-            if (par >= 0 && lineage.empty()) return fail("tree nodes are not in DFS visit order");
-            lineage.push_back(x);
-            const uint32_t len = d->h_node_len[v];
-            if (par < 0) {
-                if (root_trim[i] >= len) return fail("root_trim leaves no base of the root");
-                prob_bases[i] += len - root_trim[i];
-            } else prob_bases[i] += len;
-            if (lineage.size() > TAIL_D_CAP) return fail("tree deeper than 511 levels");
-            prob_depth[i] = std::max<uint32_t>(prob_depth[i], (uint32_t)lineage.size() - 1);
-        }
-    }
-    int rc;
-    if ((rc = query_columns(max_q, Lc))) return rc;
-    GB_CUDA(cudaSetDevice(d->device));
-    DevBuf<int32_t> d_par; DevBuf<uint32_t> d_node, d_trim, d_gap, d_counter; DevBuf<uint64_t> d_toff, d_qoff;
-    DevBuf<uint8_t> d_q, d_ws; SeamOutBufs out;
-    const uint64_t nt = tree_off[n], nq = query_off[n];
-    if ((rc = d_par.upload(tree_parent, nt ? nt : 1, d->stream, nt))) return rc;
-    if ((rc = d_node.upload(tree_node, nt ? nt : 1, d->stream, nt))) return rc;
-    if ((rc = d_toff.upload(tree_off, n + 1, d->stream))) return rc;
-    if ((rc = d_trim.upload(root_trim, n, d->stream))) return rc;
-    if ((rc = d_gap.upload(max_gap, n, d->stream))) return rc;
-    if ((rc = d_q.upload(query, nq ? nq : 1, d->stream, nq))) return rc;
-    if ((rc = d_qoff.upload(query_off, n + 1, d->stream))) return rc;
-    if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
-    if ((rc = d_counter.reserve(4))) return rc;
-    GB_CUDA(cudaMemsetAsync(d_counter.ptr, 0, 16, d->stream));
-    const size_t smem = dp_smem_per_warp(Lc) * ALIGN_WARPS;
-    if (smem > 48 * 1024) GB_CUDA(cudaFuncSetAttribute(xdrop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    uint32_t grid = std::min<uint32_t>((uint32_t)d->n_sms * 2, (n + ALIGN_WARPS - 1) / ALIGN_WARPS);
-    const uint32_t tb_cells = 2 * 1024 * 1024;
-    const size_t ws_stride = tail_ws_bytes(Lc, tb_cells);
-    if ((rc = d_ws.reserve(ws_stride * grid * ALIGN_WARPS))) return rc;
-    XdropBatch b;
-    b.tree_parent = d_par.ptr; b.tree_node = d_node.ptr; b.tree_off = d_toff.ptr; b.root_trim = d_trim.ptr;
-    b.query = d_q.ptr; b.query_off = d_qoff.ptr; b.max_gap = d_gap.ptr; b.n = n; b.Lc = Lc; b.out = out.view;
-    b.ws_base = d_ws.ptr; b.ws_stride = ws_stride; b.tb_cells = tb_cells;
-    b.work_counter = d_counter.ptr;
-    // ---- problems the int16 tile kernel can hold run there (the production path of the tails); the rest on the int32 sweep ----
-    std::vector<uint8_t> elig(n, 0); std::vector<uint32_t> toff(n, 0);
-    uint64_t units = 0; uint32_t n_elig = 0;
-    if (d->use_tiles) {
-        for (uint32_t i = 0; i < n; i++) {
-            const uint32_t ntree = (uint32_t)(tree_off[i + 1] - tree_off[i]), m = (uint32_t)(query_off[i + 1] - query_off[i]);
-            const uint32_t bases = (uint32_t)std::min<uint64_t>(prob_bases[i], 0xffffffffu);
-            if (!tile_eligible(d->sc, m, std::max(max_gap[i], 1u), ntree, bases, prob_depth[i])) continue;
-            elig[i] = 1; toff[i] = (uint32_t)units; units += tile_bytes(ntree, bases, m) / 16; n_elig++;
-        }
-    }
-    DevBuf<uint8_t> d_elig, d_tiles; DevBuf<uint32_t> d_tileoff, d_lists, d_tc, d_paths; DevBuf<TileResult> d_res;
-    GB_CUDA(cudaEventRecord(d->ev0, d->stream));
-    if (n_elig) {
-        const uint32_t path_cap = (uint32_t)std::min<uint64_t>((uint64_t)n * (2 * TILE_MAP_CAP + TILE_EDIT_CAP), 0xfffffff0ull);
-        if ((rc = d_elig.upload(elig.data(), n, d->stream)) || (rc = d_tileoff.upload(toff.data(), n, d->stream)) || (rc = d_tiles.reserve(units * 16 + 16)) ||
-            (rc = d_lists.reserve(TILE_CLASSES * (size_t)n)) || (rc = d_tc.reserve(32)) || (rc = d_res.reserve(n)) || (rc = d_paths.reserve(path_cap))) return rc;
-        GB_CUDA(cudaMemsetAsync(d_tc.ptr, 0, 128, d->stream));
-        GB_CUDA(cudaMemsetAsync(d_res.ptr, 0xff, sizeof(TileResult) * (size_t)n, d->stream));
-        PackBatch pk;
-        pk.tree_parent = d_par.ptr; pk.tree_node = d_node.ptr; pk.tree_off = d_toff.ptr; pk.root_trim = d_trim.ptr;
-        pk.query = d_q.ptr; pk.query_off = d_qoff.ptr; pk.max_gap = d_gap.ptr; pk.n = n; pk.tiles = d_tiles.ptr; pk.tile_off = d_tileoff.ptr;
-        for (int c = 0; c < TILE_CLASSES; c++) pk.lists[c] = d_lists.ptr + (size_t)c * n;
-        pk.list_count = d_tc.ptr; pk.eligible = d_elig.ptr;
-        pack_tiles_kernel<<<(n + 7) / 8, 256, 0, d->stream>>>(d->ix, d->sc, pk);
-        d->launches++;
-        GB_CUDA(cudaGetLastError());
-        d->kt_reset();
-        if ((rc = launch_tile_kernels(d, d_tiles.ptr, d_tileoff.ptr, d_lists.ptr, n, d_tc.ptr, d_tc.ptr + 8, d_res.ptr, d_paths.ptr, path_cap, d_tc.ptr + 16))) return rc;
-        b.skip = d_elig.ptr;
-        unpack_tile_results_kernel<<<(n + 7) / 8, 256, 0, d->stream>>>(b, d_res.ptr, d_paths.ptr);
-        d->launches++;
-        GB_CUDA(cudaGetLastError());
-    } else b.skip = nullptr;
-    // the int32 sweep takes the problems not eligible for a tile and those whose tile ended FULL; the latter are known only
-    // on the device, so it runs after the tiles too and skips the problems they finished
-    xdrop_kernel<<<grid, ALIGN_WARPS * 32, smem, d->stream>>>(d->ix, d->sc, b);
-    d->launches++;
-    GB_CUDA(cudaGetLastError());
-    d->last_tile_problems = n_elig;
-    GB_CUDA(cudaEventRecord(d->ev1, d->stream));
-    return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
 }

@@ -1,6 +1,7 @@
 // map_paired.cuh — paired-end kernels (included by map.cu inside namespace gb).
-//   MinimizerMapper::map_paired, minimizer_mapper.cpp:1462-2942, forced fragment distribution,
-//   max_rescue_attempts = 0 (the rescue branch, SURVEY.md §8 a17, is not built in this round).
+//   MinimizerMapper::map_paired, minimizer_mapper.cpp:1462-2942, forced fragment distribution.  With
+//   max_rescue_attempts != 0, pairs left with unpaired alignments go to the rescue build of align_kernel_pe
+//   (rescue.cuh, SURVEY.md §8 a17).
 #pragma once
 
 // Mate 2 is mapped "rightward": reverse-complemented sequence, reversed qualities (:1503-1506).
@@ -118,17 +119,11 @@ align_kernel_pe(DevIndex ix, MapParamsDev P, DevScores sc, MapBatch b, AlignArgs
     extern __shared__ __align__(16) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t gwarp = blockIdx.x * ALIGN_WARPS + warp;
-    const uint32_t W = b.Lc + 1;
-    // shared per warp: 2 reads, 2 quals, query buffer, 4 DP columns
-    const size_t bytes_part = ((size_t)b.Lc * 5 + 15) & ~(size_t)15;
-    const size_t per_warp = bytes_part + (size_t)W * 4 * 4 + 64 + a.tmp_bytes;
-    uint8_t* base = smem + (size_t)warp * per_warp;
-    uint8_t* stmp = a.tmp_bytes ? base + bytes_part + (size_t)W * 4 * 4 + 64 : nullptr;
-    uint8_t* sread[2] = {base, base + b.Lc};
-    uint8_t* squal[2] = {base + 2 * (size_t)b.Lc, base + 3 * (size_t)b.Lc};
-    uint8_t* qbuf = base + 4 * (size_t)b.Lc;
-    int32_t* cols = reinterpret_cast<int32_t*>(base + bytes_part);
-    DpSmem dps; dps.Hp = cols; dps.Ep = cols + W; dps.Hc = cols + 2 * W; dps.Ec = cols + 3 * W;
+    const AlignSmem sm = align_smem_carve(smem, warp, b.Lc, 2, a.tmp_bytes);
+    uint8_t* sread[2] = {sm.read[0], sm.read[1]};
+    uint8_t* squal[2] = {sm.qual[0], sm.qual[1]};
+    uint8_t* qbuf = sm.qbuf; uint8_t* stmp = sm.tmp;
+    const DpSmem dps = sm.dps;
     const TailWs ws = carve_tail_ws(a.ws_base + (size_t)gwarp * a.ws_stride, b.Lc, a.tb_cells);
     uint8_t* cand_base = a.cand_base + (size_t)gwarp * a.cand_stride;
     const uint32_t n_pairs = b.n_reads / 2;

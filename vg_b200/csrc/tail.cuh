@@ -189,14 +189,17 @@ struct DpSmem { int32_t *Hp, *Ep, *Hc, *Ec; };
 __host__ __device__ inline size_t dp_smem_per_warp(uint32_t Lc) {
     return (((size_t)Lc + 15) & ~(size_t)15) + ((size_t)Lc + 1) * 4 * 4 + 64;
 }
+// the four DP columns at `cols`
+__device__ inline DpSmem dp_cols_carve(int32_t* cols, uint32_t Lc) {
+    const uint32_t W = Lc + 1;
+    DpSmem dps; dps.Hp = cols; dps.Ep = cols + W; dps.Hc = cols + 2 * W; dps.Ec = cols + 3 * W;
+    return dps;
+}
 // warp `warp`'s query buffer (q) and DP columns within that layout
 __device__ inline DpSmem dp_smem_carve(uint8_t* smem, int warp, uint32_t Lc, uint8_t*& q) {
     uint8_t* base = smem + (size_t)warp * dp_smem_per_warp(Lc);
     q = base;
-    int32_t* cols = reinterpret_cast<int32_t*>(base + (((size_t)Lc + 15) & ~(size_t)15));
-    const uint32_t W = Lc + 1;
-    DpSmem dps; dps.Hp = cols; dps.Ep = cols + W; dps.Hc = cols + 2 * W; dps.Ec = cols + 3 * W;
-    return dps;
+    return dp_cols_carve(reinterpret_cast<int32_t*>(base + (((size_t)Lc + 15) & ~(size_t)15)), Lc);
 }
 
 __device__ inline int32_t xdrop_tree(const DevIndex& ix, const DevScores& sc, const TailWs& ws, DpSmem dps,

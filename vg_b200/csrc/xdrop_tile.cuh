@@ -630,48 +630,9 @@ struct PlanView {
 };
 struct TailLookup { const PlanView* pv; uint32_t base, count, key; };     // pv == nullptr: no plan (always in place)
 
-// ---- stage seam: build tiles from explicit trees (gb_xdrop_pinned_batch) ---------------------------------------------
-struct PackBatch {
-    const int32_t* tree_parent; const uint32_t* tree_node; const uint64_t* tree_off; const uint32_t* root_trim;
-    const uint8_t* query; const uint64_t* query_off; const uint32_t* max_gap; uint32_t n;
-    uint8_t* tiles; const uint32_t* tile_off;      // precomputed on the host
-    uint32_t* lists[TILE_CLASSES]; uint32_t* list_count;      // [TILE_CLASSES]
-    uint8_t* eligible;                              // [n] 0: not a tile problem (host falls back to the int32 kernel)
-};
-static __global__ void pack_tiles_kernel(DevIndex ix, DevScores sc, PackBatch b) {
-    const uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (p >= b.n || !b.eligible[p]) return;
-    const uint64_t t0 = b.tree_off[p]; const uint32_t nt = (uint32_t)(b.tree_off[p + 1] - t0);
-    const uint64_t q0 = b.query_off[p]; const uint32_t m = (uint32_t)(b.query_off[p + 1] - q0);
-    uint8_t* tile = b.tiles + (size_t)b.tile_off[p] * 16;
-    TileNode* nodes = reinterpret_cast<TileNode*>(tile + 32);
-    uint32_t n_bases = 0;
-    for (uint32_t i = 0; i < nt; i++) {                       // sequential prefix (small trees; the stage seam is not a hot path)
-        const uint32_t v = b.tree_node[t0 + i];
-        const gb_node_rec nr = load_node(ix, v);
-        const uint32_t trim = b.tree_parent[t0 + i] < 0 ? b.root_trim[p] : 0u;
-        if (lane == 0) { TileNode tn; tn.parent = b.tree_parent[t0 + i] < 0 ? 0xffffu : (uint16_t)b.tree_parent[t0 + i]; tn.len = (uint16_t)(nr.len - trim); tn.node = v; nodes[i] = tn; }
-        n_bases += nr.len - trim;
-    }
-    uint8_t* bases = tile + 32 + 8 * ((nt + 1u) & ~1u);
-    uint32_t at = 0;
-    for (uint32_t i = 0; i < nt; i++) {
-        const uint32_t v = b.tree_node[t0 + i];
-        const gb_node_rec nr = load_node(ix, v);
-        const uint32_t trim = b.tree_parent[t0 + i] < 0 ? b.root_trim[p] : 0u;
-        for (uint32_t x = lane; x < nr.len - trim; x += 32) bases[at + x] = __ldg(ix.seq + nr.seq_off + trim + x);
-        at += nr.len - trim;
-    }
-    uint8_t* q = bases + ((n_bases + 15u) & ~15u);
-    for (uint32_t x = lane; x < m; x += 32) q[x] = dp_query_base(b.query[q0 + x]);
-    if (lane == 0) {
-        TileHeader hd; hd.m = m; hd.n_nodes = nt; hd.n_bases = n_bases; hd.max_gap = max(b.max_gap[p], 1u); hd.flags = GB_TILE_TREE_SPACE;
-        hd.root_trim = b.root_trim[p]; hd.bytes = tile_bytes(nt, n_bases, m); hd.result = p;
-        *reinterpret_cast<TileHeader*>(tile) = hd;
-        const int cls = tile_class(m);
-        b.lists[cls][atomicAdd(&b.list_count[cls], 1u)] = p;
-    }
-}
+// Runs xdrop_tile_kernel over one wave of tiles: one launch per size class c over lists[c * list_cap ..], with its list
+// count at list_count[c] and its work counter at work[c] (map.cu, the only file that instantiates the kernel).
+int launch_tile_kernels(gb_device* d, const uint8_t* tiles, const uint32_t* tile_off, const uint32_t* lists, size_t list_cap,
+                        const uint32_t* list_count, uint32_t* work, TileResult* results, uint32_t* paths, uint32_t path_cap, uint32_t* path_cursor);
 
 } // namespace gb

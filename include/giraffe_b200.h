@@ -455,6 +455,26 @@ int gb_emit_gam(const gb_flat_index* ix, uint32_t n, const gb_alignment* aln, co
  * GB_ERR_CAPACITY when `out` is too small (in_bytes + 128 * (in_bytes / 0xff00 + 2) always suffices). */
 int gb_bgzf_compress(const void* in, uint64_t in_bytes, int level, void* out, uint64_t out_cap, uint64_t* out_used);
 
+/* GAF and GAM formatted on the GPU: gb_emit_gaf / gb_emit_gam for records that are already in HBM (gb_map_batch_device's
+ * outputs, or any records copied there).  Every array is a DEVICE address; node lengths and reference bases come from the
+ * handle's copy of the graph.  For the same records the bytes written to d_out are exactly those the host emitter writes:
+ * any subset or order of records (read_id selects the read), GB_ALN_ABSENT ranks skipped, read<i> names when d_names is
+ * NULL, bq:Z and the GAM quality field only when d_quals is non-NULL, GAM groups of 1000 present records.
+ *   GB_ERR_ARG       a record the host emitter refuses (decided on the device; nothing is written)
+ *   GB_ERR_CAPACITY  out_cap is too small: nothing is written and *out_used is the number of bytes needed, so the caller
+ *                    can resize and call again.  On success *out_used is the number of bytes written.
+ * The call runs on the handle's stream and synchronises once, after sizing every record: the total decides whether the
+ * fill runs.  The fill itself is left enqueued on the stream; work ordered after it there (a copy of d_out to the host,
+ * gb_device_synchronize) sees the bytes.  The output is uncompressed: gb_bgzf_compress applies to it once copied to the host. */
+int gb_emit_gaf_device(gb_device* dev, uint32_t n, const gb_alignment* d_aln, const gb_mapping* d_mappings, uint64_t mapping_pool_len,
+                       const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
+                       const uint64_t* d_read_off, const uint8_t* d_names, const uint64_t* d_name_off,
+                       char* d_out, uint64_t out_cap, uint64_t* out_used);
+int gb_emit_gam_device(gb_device* dev, uint32_t n, const gb_alignment* d_aln, const gb_mapping* d_mappings, uint64_t mapping_pool_len,
+                       const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
+                       const uint64_t* d_read_off, const uint8_t* d_names, const uint64_t* d_name_off,
+                       char* d_out, uint64_t out_cap, uint64_t* out_used);
+
 /* Device-pointer variant of both (paired != 0 selects map_paired): every pointer is a DEVICE
  * address (inputs already resident in HBM, outputs stay in HBM); all reads are at most
  * max_read_len long; d_aln holds n_reads * p->max_multimaps records (rank-major, as gb_map_batch);

@@ -217,6 +217,9 @@ def load_library() -> C.CDLL:
     for fn in (lib.gb_emit_gaf, lib.gb_emit_json, lib.gb_emit_gam):
         fn.argtypes = [C.POINTER(FlatIndex), u32, vp, vp, u64, vp, u64, u32, vp, vp, vp, vp, vp, vp, u64, vp]
         fn.restype = C.c_int
+    for fn in (lib.gb_emit_gaf_device, lib.gb_emit_gam_device):
+        fn.argtypes = [vp, u32, vp, vp, u64, vp, u64, u32, vp, vp, vp, vp, vp, vp, u64, vp]
+        fn.restype = C.c_int
     lib.gb_debug_seed_stage.argtypes = [vp, C.POINTER(MapParams), C.c_int, u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, u64]
     lib.gb_debug_seed_stage.restype = C.c_int
     lib.gb_device_pool_overflow.argtypes = [vp, C.POINTER(C.c_int)]
@@ -494,6 +497,18 @@ def emit_text(kind, flat_index, aln, maps, edits, rbuf, qbuf, read_off, names=No
     if rc != GB_OK:
         raise GbError(rc, "gb_emit_" + kind)
     data = out[: used.value].tobytes()
+    return data if kind == "gam" else data.decode()
+
+
+def emit_device_text(dev, kind, aln, maps, edits, reads, read_off, quals=None, names=None):
+    """Device.emit_device over CUDA tensors, returned like emit_text (str for GAF, bytes for GAM); names: optional list of str."""
+    import torch
+    nbuf = noff = None
+    if names is not None:
+        enc = [s.encode() for s in names]
+        noff = torch.tensor(np.concatenate([[0], np.cumsum([len(b) for b in enc])]).astype(np.int64), device=reads.device)
+        nbuf = torch.frombuffer(bytearray(b"".join(enc) + b"\0"), dtype=torch.uint8).to(reads.device)
+    data = dev.emit_device(kind, aln, maps, edits, reads, read_off, quals, nbuf, noff).cpu().numpy().tobytes()
     return data if kind == "gam" else data.decode()
 
 
@@ -874,6 +889,35 @@ class Device:
         if rc != GB_OK:
             raise GbError(rc, "gb_stage_times")
         return [float(x) for x in ms]
+
+    def emit_device(self, kind, aln, maps, edits, reads, read_off, quals=None, names=None, name_off=None, out=None):
+        """gb_emit_gaf_device / gb_emit_gam_device (kind = "gaf" | "gam") over CUDA tensors: aln = the 32-byte records (any
+        shape / dtype, contiguous), maps = the 8-byte mappings, edits = 32-bit edit words, reads / quals (may be None) = bytes
+        addressed by read_off (int64, n_reads + 1), names (uint8) / name_off (int64, n_reads + 1) or None for read<i>.
+        Returns the formatted bytes as a uint8 CUDA tensor, a view of `out` when `out` is large enough (otherwise a new
+        tensor of the size the first call reported).  The inputs are waited for on the current torch stream, and the
+        result is complete when this returns."""
+        import torch
+        lib = load_library()
+        fn = {"gaf": lib.gb_emit_gaf_device, "gam": lib.gb_emit_gam_device}[kind]
+        vp = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+        n, n_maps, n_edits = aln.numel() * aln.element_size() // 32, maps.numel() * maps.element_size() // 8, edits.numel() * edits.element_size() // 4
+        torch.cuda.current_stream(reads.device).synchronize()
+        if out is None:
+            out = torch.empty(1, dtype=torch.uint8, device=reads.device)
+        used = C.c_uint64()
+        for attempt in range(2):
+            rc = fn(self._h, n, vp(aln), vp(maps), n_maps, vp(edits), n_edits, read_off.numel() - 1, vp(reads), vp(quals), vp(read_off),
+                    vp(names), vp(name_off), vp(out), out.numel(), C.byref(used))
+            if rc != GB_ERR_CAPACITY or attempt:
+                break
+            out = torch.empty(max(1, used.value), dtype=torch.uint8, device=reads.device)
+        if rc != GB_OK:
+            raise GbError(rc, "gb_emit_" + kind + "_device")
+        rc = lib.gb_device_synchronize(self._h)
+        if rc != GB_OK:
+            raise GbError(rc, "gb_device_synchronize")
+        return out[: used.value]
 
     def close(self):
         if getattr(self, "_h", None):

@@ -465,7 +465,8 @@ int gb_bgzf_compress(const void* in, uint64_t in_bytes, int level, void* out, ui
  *                    can resize and call again.  On success *out_used is the number of bytes written.
  * The call runs on the handle's stream and synchronises once, after sizing every record: the total decides whether the
  * fill runs.  The fill itself is left enqueued on the stream; work ordered after it there (a copy of d_out to the host,
- * gb_device_synchronize) sees the bytes.  The output is uncompressed: gb_bgzf_compress applies to it once copied to the host. */
+ * gb_device_synchronize) sees the bytes.  The output is uncompressed: gb_bgzf_compress_device compresses it without leaving HBM
+ * (or gb_bgzf_compress once it is copied to the host). */
 int gb_emit_gaf_device(gb_device* dev, uint32_t n, const gb_alignment* d_aln, const gb_mapping* d_mappings, uint64_t mapping_pool_len,
                        const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
                        const uint64_t* d_read_off, const uint8_t* d_names, const uint64_t* d_name_off,
@@ -474,6 +475,21 @@ int gb_emit_gam_device(gb_device* dev, uint32_t n, const gb_alignment* d_aln, co
                        const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
                        const uint64_t* d_read_off, const uint8_t* d_names, const uint64_t* d_name_off,
                        char* d_out, uint64_t out_cap, uint64_t* out_used);
+
+/* BGZF on the GPU: the container gb_bgzf_compress writes, for bytes already in HBM (gb_emit_gam_device / gb_emit_gaf_device
+ * output, or any other bytes).  d_in and d_out are DEVICE addresses; d_in may start at any byte.  The input is cut every
+ * 0xff00 bytes exactly as gb_bgzf_compress cuts it (so BGZF virtual offsets agree); every block is one gzip member with the
+ * host's 16 header bytes, BSIZE - 1, a raw deflate payload, CRC32 and ISIZE, and the stream ends with the same 28-byte EOF
+ * block (an empty input gives only that block).  The payload is the device's own: one dynamic-Huffman deflate block per
+ * BGZF block, or a stored block when that would not be smaller, so it is not zlib's bytes, but any inflater reads it and
+ * the same input gives the same bytes on every call.  There is no level: the device has one compressor.
+ *   GB_ERR_ARG       dev or out_used is NULL, d_out is NULL, or d_in is NULL with in_bytes > 0
+ *   GB_ERR_CAPACITY  out_cap is too small: nothing is written to d_out and *out_used is the number of bytes needed.
+ *                    in_bytes + 128 * (in_bytes / 0xff00 + 2), gb_bgzf_compress's bound, always suffices.
+ * The call runs on the handle's stream and synchronises once, for the total size; the gather into d_out is left enqueued
+ * there, like the fill of gb_emit_*_device.  Workspace on the handle (kept between calls, grown on demand): 64 KiB per
+ * input block (about 1.004 x in_bytes) plus 255 KiB per SM for the parsed tokens (34 MB on a 132-SM H100). */
+int gb_bgzf_compress_device(gb_device* dev, const void* d_in, uint64_t in_bytes, void* d_out, uint64_t out_cap, uint64_t* out_used);
 
 /* Device-pointer variant of both (paired != 0 selects map_paired): every pointer is a DEVICE
  * address (inputs already resident in HBM, outputs stay in HBM); all reads are at most

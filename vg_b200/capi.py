@@ -232,6 +232,8 @@ def load_library() -> C.CDLL:
     lib.gb_plan_stats.restype = C.c_int
     lib.gb_bgzf_compress.argtypes = [vp, u64, C.c_int, vp, u64, vp]
     lib.gb_bgzf_compress.restype = C.c_int
+    lib.gb_bgzf_compress_device.argtypes = [vp, vp, u64, vp, u64, vp]
+    lib.gb_bgzf_compress_device.restype = C.c_int
     lib.gb_last_kernel_ms.argtypes = [vp]
     lib.gb_last_kernel_ms.restype = C.c_float
     lib.gb_launch_count.argtypes = [vp]
@@ -914,6 +916,30 @@ class Device:
             out = torch.empty(max(1, used.value), dtype=torch.uint8, device=reads.device)
         if rc != GB_OK:
             raise GbError(rc, "gb_emit_" + kind + "_device")
+        rc = lib.gb_device_synchronize(self._h)
+        if rc != GB_OK:
+            raise GbError(rc, "gb_device_synchronize")
+        return out[: used.value]
+
+    def bgzf_compress_device(self, data, out=None):
+        """gb_bgzf_compress_device over a uint8 CUDA tensor (any offset, contiguous): the BGZF stream as a uint8 CUDA tensor,
+        a view of `out` when `out` is large enough (otherwise a new tensor of the size the first call reported).  The input
+        is waited for on the current torch stream, and the result is complete when this returns."""
+        import torch
+        lib = load_library()
+        assert data.dtype == torch.uint8 and data.is_cuda and data.is_contiguous()
+        torch.cuda.current_stream(data.device).synchronize()
+        if out is None:
+            out = torch.empty(1, dtype=torch.uint8, device=data.device)
+        used = C.c_uint64()
+        for attempt in range(2):
+            rc = lib.gb_bgzf_compress_device(self._h, C.c_void_p(data.data_ptr()) if data.numel() else None, data.numel(),
+                                             C.c_void_p(out.data_ptr()), out.numel(), C.byref(used))
+            if rc != GB_ERR_CAPACITY or attempt:
+                break
+            out = torch.empty(used.value, dtype=torch.uint8, device=data.device)
+        if rc != GB_OK:
+            raise GbError(rc, "gb_bgzf_compress_device")
         rc = lib.gb_device_synchronize(self._h)
         if rc != GB_OK:
             raise GbError(rc, "gb_device_synchronize")

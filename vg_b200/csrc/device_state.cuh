@@ -173,4 +173,5 @@ struct gb_device {
     gb::DevBuf<uint64_t> c_run;            // running mapping / edit totals of a host-buffer call
     uint32_t map_chunk = 1u << 20;         // reads per chunk; GIRAFFE_B200_MAP_CHUNK overrides
     gb::DevBuf<uint8_t> emit_ws;           // gb_emit_*_device: per-record sizes, offsets, scan temporaries
+    gb::DevBuf<uint8_t> bgzf_ws;           // gb_bgzf_compress_device: member slots, token slots, member sizes and offsets
 };

@@ -491,6 +491,65 @@ int gb_emit_gam_device(gb_device* dev, uint32_t n, const gb_alignment* d_aln, co
  * input block (about 1.004 x in_bytes) plus 255 KiB per SM for the parsed tokens (34 MB on a 132-SM H100). */
 int gb_bgzf_compress_device(gb_device* dev, const void* d_in, uint64_t in_bytes, void* d_out, uint64_t out_cap, uint64_t* out_used);
 
+/* BGZF inflated on the GPU, the inverse of gb_bgzf_compress_device: the whole BGZF members at the start of d_in (a DEVICE
+ * address, any byte alignment) are inflated into d_out (DEVICE), one after the other.  A member is a gzip header whose FLG is
+ * FEXTRA alone (FNAME, FCOMMENT and FHCRC are refused) with a 'BC' subfield of SLEN 2 anywhere among its XLEN bytes; BSIZE
+ * gives its length; its raw deflate payload (stored, fixed and dynamic blocks) must end with its BFINAL block in the
+ * payload's last byte; CRC32 and ISIZE must match the inflated bytes and ISIZE must be at most 65536; back-references may not
+ * reach before the member's own output.  A member is accepted exactly when zlib's raw inflate accepts its payload with
+ * nothing left over and the trailer matches, and the output is then zlib's bytes.  Empty members (the 28-byte EOF block) are
+ * accepted anywhere, so concatenated bgzip files work.
+ *   final == 0  a member that runs past in_bytes ends the call without error: *in_used is its first byte, and the caller
+ *               passes the bytes from there again, followed by more input, in its next call
+ *   final != 0  such a member is GB_ERR_FORMAT
+ *   GB_ERR_FORMAT    not BGZF (gb_last_error() names the byte offset), including single-member gzip without the 'BC'
+ *                    subfield (plain `gzip` output), which cannot be split into blocks: inflate such a file on the host.
+ *                    After it, the contents of d_out are unspecified.
+ *   GB_ERR_CAPACITY  out_cap is below the sum of the ISIZEs (read from the trailers before anything is inflated): nothing is
+ *                    written and *out_used is the number of bytes needed.
+ * On success *out_used is the number of bytes written and *in_used the bytes of d_in consumed.  The call runs on the
+ * handle's stream and waits twice: once for the member walk (count, sizes, where it stopped), once for the inflate status.
+ * Workspace on the handle (kept, grown on demand): 32 bytes per 26 input bytes in the worst case (the member list). */
+int gb_bgzf_decompress_device(gb_device* dev, const void* d_in, uint64_t in_bytes, int final,
+                              void* d_out, uint64_t out_cap, uint64_t* out_used, uint64_t* in_used);
+
+/* FASTQ parsed on the GPU into the arrays gb_map_batch_device and gb_emit_{gaf,gam}_device take: bases and qualities
+ * concatenated and addressed by d_read_off[n + 1], names concatenated and addressed by d_name_off[n + 1] (all DEVICE).
+ * d_text is a HOST array of n_inputs DEVICE pointers, each starting at a record boundary:
+ *   n_inputs 1              single-end: record i is read i
+ *   n_inputs 1, flags GB_FASTQ_INTERLEAVED   records 2i and 2i + 1 are mates 1 and 2 (vg giraffe -i)
+ *   n_inputs 2              record i of input 0 is read 2i, record i of input 1 read 2i + 1 (vg giraffe -f r1 -f r2): the
+ *                           mate order gb_map_batch_device(paired = 1) expects
+ * Per record, vg's reader (get_next_alignment_from_fastq, src/alignment.cpp:159-250; giraffe_main.cpp:2319, :2433):
+ *   name       the bytes after '@' up to the first of " \t\v\f\r" or the line end (the comment is dropped, /1 and /2 are
+ *              kept; may be empty)
+ *   sequence   the second line (one line); 'a'..'z' uppercased, every other byte unchanged
+ *   separator  the third line, which must start with '+' (its rest is not looked at)
+ *   quality    the fourth line, each byte - 33 (raw Phred, as vg's Alignment.quality holds it); d_quals may be NULL
+ * The call takes whole records (whole pairs when paired) in input order and stops, without error, at the first that is not
+ * complete in the text or does not fit max_reads, bases_cap or names_cap.  *n_reads, *max_read_len (the longest read taken)
+ * and text_used[n_inputs] (bytes consumed per input) say how far it got; the caller passes the rest again, followed by more
+ * text, in its next call.  GB_ERR_CAPACITY when a complete record (pair) is present but none fits.
+ * With final != 0 the text is the end of the input: an input whose whole records were all taken must end with the last of
+ * them (bytes that do not form a complete record, such as a last line without '\n', are GB_ERR_FORMAT; vg refuses such a
+ * file too).  With two inputs the longer one's surplus records, and the odd last record of an interleaved input, are left
+ * unconsumed (text_used shows them; vg drops them silently, alignment.cpp:252-258).
+ * GB_ERR_FORMAT, with the input, record index and byte offset in gb_last_error(), for a record the call reaches whose
+ *   - header does not start with '@' (including FASTA's '>': FASTA input is not supported)
+ *   - separator line does not start with '+'
+ *   - quality length differs from the sequence length (divergence: vg also accepts an empty quality line)
+ *   - sequence or quality line holds a byte outside '!'..'~' (divergence: this refuses CRLF files and NULs, which vg passes
+ *     into the read as '\r' and as a negative quality)
+ * After GB_ERR_FORMAT the contents of the output arrays are unspecified.
+ * Not supported: multi-line FASTQ, FASTA, --comments-as-tags.  The call runs on the handle's stream and waits once, for the
+ * counts.  Workspace on the handle (kept, grown on demand): 32 bytes per line the call may look at (4 * max_reads + 8 lines)
+ * plus 40 bytes per read of max_reads. */
+#define GB_FASTQ_INTERLEAVED 1u
+int gb_fastq_parse_device(gb_device* dev, uint32_t n_inputs, const uint8_t* const* d_text, const uint64_t* text_bytes,
+                          uint32_t flags, int final, uint32_t max_reads, uint8_t* d_reads, uint8_t* d_quals, uint64_t bases_cap,
+                          uint64_t* d_read_off, uint8_t* d_names, uint64_t names_cap, uint64_t* d_name_off,
+                          uint32_t* n_reads, uint32_t* max_read_len, uint64_t* text_used);
+
 /* Device-pointer variant of both (paired != 0 selects map_paired): every pointer is a DEVICE
  * address (inputs already resident in HBM, outputs stay in HBM); all reads are at most
  * max_read_len long; d_aln holds n_reads * p->max_multimaps records (rank-major, as gb_map_batch);

@@ -17,6 +17,7 @@ LIB_PATH = ROOT / "vg_b200" / "libgiraffe_b200.so"
 
 GB_OK = 0
 GB_ERR_ARG, GB_ERR_CUDA, GB_ERR_NO_DEVICE, GB_ERR_CAPACITY, GB_ERR_FORMAT = -1, -2, -3, -4, -5
+GB_FASTQ_INTERLEAVED = 1
 GB_ITEM_OK, GB_ITEM_QUEUE_FULL, GB_ITEM_OUT_FULL, GB_ITEM_DP_REFUSED = 0, 1, 2, 3
 GB_ITEM_NO_BAND = 4
 GB_EXT_LEFT_FULL, GB_EXT_RIGHT_FULL = 1, 2
@@ -234,6 +235,10 @@ def load_library() -> C.CDLL:
     lib.gb_bgzf_compress.restype = C.c_int
     lib.gb_bgzf_compress_device.argtypes = [vp, vp, u64, vp, u64, vp]
     lib.gb_bgzf_compress_device.restype = C.c_int
+    lib.gb_bgzf_decompress_device.argtypes = [vp, vp, u64, C.c_int, vp, u64, vp, vp]
+    lib.gb_bgzf_decompress_device.restype = C.c_int
+    lib.gb_fastq_parse_device.argtypes = [vp, u32, vp, vp, u32, C.c_int, u32, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp]
+    lib.gb_fastq_parse_device.restype = C.c_int
     lib.gb_last_kernel_ms.argtypes = [vp]
     lib.gb_last_kernel_ms.restype = C.c_float
     lib.gb_launch_count.argtypes = [vp]
@@ -944,6 +949,69 @@ class Device:
         if rc != GB_OK:
             raise GbError(rc, "gb_device_synchronize")
         return out[: used.value]
+
+    def bgzf_decompress_device(self, data, final=True, out=None):
+        """gb_bgzf_decompress_device over a uint8 CUDA tensor (any offset, contiguous): returns (inflated bytes as a uint8 CUDA
+        tensor, input bytes consumed).  The result is a view of `out` when `out` is large enough (otherwise a new tensor of
+        the size the first call reported).  final=False leaves a member cut by the end of `data` unconsumed."""
+        import torch
+        lib = load_library()
+        assert data.dtype == torch.uint8 and data.is_cuda and data.is_contiguous()
+        torch.cuda.current_stream(data.device).synchronize()
+        if out is None:
+            out = torch.empty(1, dtype=torch.uint8, device=data.device)
+        used, in_used = C.c_uint64(), C.c_uint64()
+        for attempt in range(2):
+            rc = lib.gb_bgzf_decompress_device(self._h, C.c_void_p(data.data_ptr()) if data.numel() else None, data.numel(),
+                                               1 if final else 0, C.c_void_p(out.data_ptr()), out.numel(), C.byref(used),
+                                               C.byref(in_used))
+            if rc != GB_ERR_CAPACITY or attempt:
+                break
+            out = torch.empty(max(1, used.value), dtype=torch.uint8, device=data.device)
+        if rc != GB_OK:
+            raise GbError(rc, "gb_bgzf_decompress_device")
+        return out[: used.value], in_used.value
+
+    def fastq_parse_device(self, texts, interleaved=False, final=True, max_reads=None, bases_cap=None, names_cap=None, quals=True):
+        """gb_fastq_parse_device over one or two uint8 CUDA tensors of FASTQ text.  The capacities default to what the whole
+        text could need.  Returns a dict of CUDA tensors reads, quals (None when quals=False), read_off (int64, n + 1),
+        names, name_off (int64, n + 1), and n_reads, max_read_len, text_used (list of ints)."""
+        import torch
+        lib = load_library()
+        texts = list(texts)
+        dev = texts[0].device
+        for t in texts:
+            assert t.dtype == torch.uint8 and t.is_cuda and t.is_contiguous()
+        total = sum(t.numel() for t in texts)
+        if max_reads is None:
+            max_reads = total // 3 + 2                    # a record is at least 6 bytes (4 lines)
+        if bases_cap is None:
+            bases_cap = total
+        if names_cap is None:
+            names_cap = total
+        reads = torch.empty(max(1, bases_cap), dtype=torch.uint8, device=dev)
+        q = torch.empty(max(1, bases_cap), dtype=torch.uint8, device=dev) if quals else None
+        names = torch.empty(max(1, names_cap), dtype=torch.uint8, device=dev)
+        read_off = torch.zeros(max_reads + 1, dtype=torch.int64, device=dev)
+        name_off = torch.zeros(max_reads + 1, dtype=torch.int64, device=dev)
+        ptrs = (C.c_void_p * len(texts))(*[t.data_ptr() if t.numel() else None for t in texts])
+        sizes = (C.c_uint64 * len(texts))(*[t.numel() for t in texts])
+        used = (C.c_uint64 * len(texts))()
+        n, mx = C.c_uint32(), C.c_uint32()
+        torch.cuda.current_stream(dev).synchronize()
+        rc = lib.gb_fastq_parse_device(self._h, len(texts), ptrs, sizes, GB_FASTQ_INTERLEAVED if interleaved else 0, 1 if final else 0,
+                                       max_reads, C.c_void_p(reads.data_ptr()), C.c_void_p(q.data_ptr()) if quals else None, bases_cap,
+                                       C.c_void_p(read_off.data_ptr()), C.c_void_p(names.data_ptr()), names_cap,
+                                       C.c_void_p(name_off.data_ptr()), C.byref(n), C.byref(mx), used)
+        if rc != GB_OK:
+            raise GbError(rc, "gb_fastq_parse_device")
+        rc = lib.gb_device_synchronize(self._h)
+        if rc != GB_OK:
+            raise GbError(rc, "gb_device_synchronize")
+        k = n.value
+        nb, nn = int(read_off[k]), int(name_off[k])
+        return {"reads": reads[:nb], "quals": q[:nb] if quals else None, "read_off": read_off[: k + 1], "names": names[:nn],
+                "name_off": name_off[: k + 1], "n_reads": k, "max_read_len": mx.value, "text_used": [int(x) for x in used]}
 
     def close(self):
         if getattr(self, "_h", None):

@@ -25,6 +25,7 @@
 // so the output is the same on every call.
 #include "giraffe_b200.h"
 #include "device_state.cuh"
+#include "crc32.cuh"
 
 #include <cub/cub.cuh>
 
@@ -41,7 +42,6 @@ constexpr uint32_t BGZF_CHAIN = 8;               // chain candidates tried per p
 constexpr uint32_t BGZF_NICE = 128;              // a match this long ends the chain walk
 constexpr uint32_t HASH_BITS = 13;
 constexpr uint32_t WINDOW = 32768;
-constexpr uint32_t CRC_POLY = 0xedb88320u;
 constexpr uint32_t CRC_LEVELS = 9;               // log2(BGZF_THREADS): levels of the CRC combine tree
 static_assert(1u << CRC_LEVELS == BGZF_THREADS, "one CRC slice per thread");
 
@@ -60,23 +60,6 @@ constexpr uint32_t M_NRLE = 0, M_HLIT = 1, M_HDIST = 2, M_HCLEN = 3, M_HDRBITS =
 
 __constant__ uint8_t c_cl_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
 __constant__ uint8_t c_eof[28] = {0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 'B', 'C', 2, 0, 0x1b, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-
-// ---- CRC-32 ------------------------------------------------------------------------------------------------------------
-__device__ uint32_t multmodp(uint32_t a, uint32_t b) {          // a * b mod P, bit-reflected (a != 0)
-    uint32_t m = 1u << 31, p = 0;
-    for (;;) {
-        if (a & m) { p ^= b; if ((a & (m - 1)) == 0) break; }
-        m >>= 1;
-        b = (b & 1) ? (b >> 1) ^ CRC_POLY : b >> 1;
-    }
-    return p;
-}
-__device__ uint32_t x8nmodp(uint64_t n, const uint32_t* x2n) {  // x^(8n) mod P; x2n[k] = x^(2^k)
-    uint32_t p = 1u << 31;
-    for (uint32_t k = 3; n; n >>= 1, k++)
-        if (n & 1) p = multmodp(x2n[k & 31], p);
-    return p;
-}
 
 // ---- deflate symbols ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t ilog2(uint32_t v) { return 31 - __clz(v); }
@@ -209,15 +192,7 @@ bgzf_block_kernel(const uint8_t* __restrict__ src, uint64_t in_bytes, uint64_t n
     const uint32_t t = threadIdx.x, lane = t & 31;
     // the CRC table and x^(2^k) mod P, once per CTA
     __shared__ uint32_t crc_tab[256], x2n[32], level_op[CRC_LEVELS];
-    for (uint32_t i = t; i < 256; i += BGZF_THREADS) {
-        uint32_t c = i;
-        for (int k = 0; k < 8; k++) c = (c & 1) ? (c >> 1) ^ CRC_POLY : c >> 1;
-        crc_tab[i] = c;
-    }
-    if (t == 0) {
-        x2n[0] = 1u << 30;
-        for (int k = 1; k < 32; k++) x2n[k] = multmodp(x2n[k - 1], x2n[k - 1]);
-    }
+    crc32_tables(crc_tab, x2n, t, BGZF_THREADS);
 
     for (uint64_t b = blockIdx.x; b < n_blocks; b += gridDim.x) {
         const uint64_t at = b * BGZF_BLOCK;

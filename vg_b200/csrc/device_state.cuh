@@ -174,4 +174,6 @@ struct gb_device {
     uint32_t map_chunk = 1u << 20;         // reads per chunk; GIRAFFE_B200_MAP_CHUNK overrides
     gb::DevBuf<uint8_t> emit_ws;           // gb_emit_*_device: per-record sizes, offsets, scan temporaries
     gb::DevBuf<uint8_t> bgzf_ws;           // gb_bgzf_compress_device: member slots, token slots, member sizes and offsets
+    gb::DevBuf<uint8_t> inflate_ws;        // gb_bgzf_decompress_device: the member list and the walk's summary
+    gb::DevBuf<uint8_t> fastq_ws;          // gb_fastq_parse_device: line ends, per-read lengths and offsets, scan temporaries
 };

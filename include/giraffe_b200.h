@@ -259,7 +259,16 @@ typedef struct gb_extend_params {
  *   indices into those pools.
  * Canonical order (the reference iterates an unordered set, gbwt_extender.cpp:550): seeds
  * are processed in ascending (node, diag) order and ties in the full-length sort
- * (gbwt_extender.cpp:302) keep that order (stable). */
+ * (gbwt_extender.cpp:302) keep that order (stable).
+ * Seeds the reference would read out of bounds with are skipped: a node v outside [2, n_nodes) or of length 0, a
+ * read offset max(diag, 0) past the end of the read, or a node offset max(-diag, 0) past the end of the node.  Offsets
+ * equal to the read or node length are valid (an empty initial match).
+ * Limits: reads of up to 25600 bases (8 warps x read length of shared memory, at most 200 KiB; a longer read returns
+ * GB_ERR_ARG before anything is launched); per warp, a best-first frontier of 511 entries and 4096 path-arena nodes
+ * per seed (GB_ITEM_QUEUE_FULL past either); per item, max_ext_per_item raw records (one per extended seed, before
+ * duplicates are removed), path_cap_per_item nodes over those records and mism_cap_per_item mismatches over the
+ * records left after the full-length or duplicate filter, before trimming (GB_ITEM_OUT_FULL past any).  An item
+ * refused this way has ext_count 0. */
 int gb_extend_batch(gb_device* dev, const gb_extend_params* p,
                     uint32_t n_reads, const uint8_t* reads, const uint64_t* read_off,
                     uint32_t n_items, const uint32_t* item_read,

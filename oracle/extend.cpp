@@ -195,11 +195,25 @@ bool trim_mismatches(GaplessExtension& e, const Graph& g, const gb_scores& s) {
 
 } // namespace
 
-// gbwt_extender.cpp:533-737
+// What one call asks of the extension kernel's fixed resources (extend.cuh), and the GB_ITEM_* status the capacities
+// below give it.  Each capacity is checked where the kernel checks it, so the first one exceeded decides the status:
+//   frontier / arena   before every push of the search (extend.cuh extend_search: qn + 1 >= q_cap, an >= a_cap)
+//   records / paths    when a seed's best match is added to the result
+//   mismatch pool      after the full-length or duplicate filter, before trimming (extend_finish)
+struct ExtendTrace {
+    uint64_t q_cap = UINT64_MAX, a_cap = UINT64_MAX, max_ext = UINT64_MAX, path_cap = UINT64_MAX, mism_cap = UINT64_MAX;
+    int status = GB_ITEM_OK;
+    uint64_t records = 0, path_nodes = 0, mismatches = 0, peak_frontier = 0, peak_arena = 0;
+    std::set<std::pair<uint32_t, int64_t>> contained, invalid;    // seeds skipped, by reason
+    void fail(int s) { if (status == GB_ITEM_OK) status = s; }
+};
+
+// gbwt_extender.cpp:533-737.  Seeds the reference would read out of bounds with (a node that is not in the graph or
+// is empty, a read offset past the read, a node offset past the node) are skipped, as in extend.cuh.
 std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
                                      const std::vector<std::pair<uint32_t, int64_t>>& cluster_in,
                                      std::string sequence, size_t max_mismatches,
-                                     double overlap_threshold, bool trim) {
+                                     double overlap_threshold, bool trim, ExtendTrace* trace) {
     std::vector<GaplessExtension> result;
     if (cluster_in.empty() || sequence.empty()) return result;
     // ReadMasker("ACGT"), gbwt_extender.cpp:160-170
@@ -209,8 +223,19 @@ std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
 
     size_t best_alignment = std::numeric_limits<size_t>::max();
     for (auto seed : cluster) {
+        {
+            const size_t read_offset = seed.second < 0 ? 0 : (size_t)seed.second;
+            const size_t node_offset = seed.second < 0 ? (size_t)(-seed.second) : 0;
+            if (!g.has_node(seed.first) || read_offset > sequence.length() || node_offset > g.get_length(seed.first)) {
+                if (trace) trace->invalid.insert(seed);
+                continue;
+            }
+        }
         if (best_alignment < result.size() && result[best_alignment].internal_score == 0) {
-            if (result[best_alignment].contains(g, seed.first, seed.second)) continue;
+            if (result[best_alignment].contains(g, seed.first, seed.second)) {
+                if (trace) trace->contained.insert(seed);
+                continue;
+            }
         }
         GaplessExtension best_match;
         best_match.score = std::numeric_limits<int32_t>::min();
@@ -225,6 +250,15 @@ std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
         };
         std::priority_queue<queue_item, std::vector<queue_item>, decltype(cmp)> extensions(cmp);
         size_t extension_number = 0;
+        uint64_t arena = 0;              // extensions pushed for this seed: the kernel's parent-pointer arena
+        // the kernel's check before pushing a new extension (arena node + frontier entry) or a re-pushed one (entry only)
+        auto before_push = [&](bool new_node) {
+            if (!trace) return;
+            if ((new_node && arena >= trace->a_cap) || extensions.size() + 1 >= trace->q_cap) trace->fail(GB_ITEM_QUEUE_FULL);
+            arena += new_node;
+            trace->peak_arena = std::max(trace->peak_arena, arena);
+            trace->peak_frontier = std::max<uint64_t>(trace->peak_frontier, extensions.size() + 1);
+        };
         {
             size_t read_offset = seed.second < 0 ? 0 : (size_t)seed.second;
             size_t node_offset = seed.second < 0 ? (size_t)(-seed.second) : 0;
@@ -238,6 +272,7 @@ std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
             if (match.read_interval.second >= sequence.length()) { match.right_full = true; match.right_maximal = true; }
             set_score(match, scores);
             extensions.emplace(std::move(match), extension_number++);
+            if (trace) trace->peak_frontier = std::max<uint64_t>(trace->peak_frontier, 1);
         }
         while (!extensions.empty()) {
             GaplessExtension curr = extensions.top().first;
@@ -264,12 +299,14 @@ std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
                     }
                     set_score(next, scores);
                     num_extensions += next.state.size();
+                    before_push(true);
                     extensions.emplace(std::move(next), extension_number++);
                     return true;
                 });
                 if (num_extensions < curr.state.size()) {
                     curr.right_maximal = true;
                     curr.old_score = curr.internal_score;
+                    before_push(false);
                     extensions.emplace(std::move(curr), extension_number++);
                 }
                 continue;
@@ -294,6 +331,7 @@ std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
                     if (next.read_interval.first == 0) { next.left_full = true; next.left_maximal = true; }
                     else if (next.offset > 0) { next.left_maximal = true; }
                     set_score(next, scores);
+                    before_push(true);
                     extensions.emplace(std::move(next), extension_number++);
                     found_extension = true;
                     return true;
@@ -304,6 +342,10 @@ std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
             if (best_match < curr) best_match = std::move(curr);
         }
         if (!best_match.empty()) {
+            if (trace) {
+                if (result.size() >= trace->max_ext || trace->path_nodes + best_match.path.size() > trace->path_cap) trace->fail(GB_ITEM_OUT_FULL);
+                trace->records++; trace->path_nodes += best_match.path.size();
+            }
             if (best_match.full() && (best_alignment >= result.size() ||
                                       best_match.internal_score < result[best_alignment].internal_score)) {
                 best_alignment = result.size();
@@ -312,12 +354,19 @@ std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
         }
     }
 
+    auto count_mismatches = [&]() {
+        if (!trace) return;
+        for (const GaplessExtension& e : result) trace->mismatches += e.mismatch_positions.size();
+        if (trace->mismatches > trace->mism_cap) trace->fail(GB_ITEM_OUT_FULL);
+    };
     if (best_alignment < result.size() && result[best_alignment].internal_score <= max_mismatches) {
         handle_full_length(g, result, overlap_threshold);
         find_mismatches(sequence, g, result);
+        count_mismatches();
     } else {
         remove_duplicates(result);
         find_mismatches(sequence, g, result);
+        count_mismatches();
         if (trim) {
             bool trimmed = false;
             for (GaplessExtension& e : result) trimmed |= trim_mismatches(e, g, scores);
@@ -340,7 +389,7 @@ extern "C" int oracle_extend(const gb_flat_index* ix, const gb_scores* scores,
     std::vector<std::pair<uint32_t, int64_t>> cluster;
     for (uint32_t i = 0; i < n_seeds; i++) cluster.emplace_back(seeds[i].node, (int64_t)seeds[i].diag);
     auto result = oracle::extend(g, *scores, cluster, std::string((const char*)read, read_len),
-                                 max_mismatches, overlap_threshold, trim != 0);
+                                 max_mismatches, overlap_threshold, trim != 0, nullptr);
     if (result.size() > max_ext) return -1;
     uint32_t pp = 0, mp = 0;
     for (size_t i = 0; i < result.size(); i++) {
@@ -360,6 +409,32 @@ extern "C" int oracle_extend(const gb_flat_index* ix, const gb_scores* scores,
         o.mismatches = (uint32_t)e.mismatch_positions.size();
     }
     return (int)result.size();
+}
+
+extern "C" int oracle_extend_limits(const gb_flat_index* ix, const gb_scores* scores,
+                                    const uint8_t* read, uint32_t read_len,
+                                    const gb_seed* seeds, uint32_t n_seeds,
+                                    uint32_t max_mismatches, double overlap_threshold, int trim,
+                                    uint32_t q_cap, uint32_t a_cap, uint32_t max_ext, uint32_t path_cap, uint32_t mism_cap,
+                                    uint64_t* needs_out, uint8_t* seed_skip) {
+    oracle::Graph g(ix);
+    std::vector<std::pair<uint32_t, int64_t>> cluster;
+    for (uint32_t i = 0; i < n_seeds; i++) cluster.emplace_back(seeds[i].node, (int64_t)seeds[i].diag);
+    oracle::ExtendTrace t;
+    t.q_cap = q_cap; t.a_cap = a_cap; t.max_ext = max_ext; t.path_cap = path_cap; t.mism_cap = mism_cap;
+    oracle::extend(g, *scores, cluster, std::string((const char*)read, read_len), max_mismatches, overlap_threshold,
+                   trim != 0, &t);
+    if (needs_out) {
+        needs_out[0] = t.records; needs_out[1] = t.path_nodes; needs_out[2] = t.mismatches;
+        needs_out[3] = t.peak_frontier; needs_out[4] = t.peak_arena;
+    }
+    if (seed_skip) {
+        for (uint32_t i = 0; i < n_seeds; i++) {
+            const auto s = cluster[i];
+            seed_skip[i] = t.invalid.count(s) ? 2 : t.contained.count(s) ? 1 : 0;
+        }
+    }
+    return t.status;
 }
 
 // GaplessExtension helpers on hand-built extensions (test entries for unittest/gbwt_extender.cpp:576-820).

@@ -17,10 +17,11 @@ namespace oracle {
 } // namespace oracle
 #include "extension.hpp"
 namespace oracle {
+struct ExtendTrace;
 std::vector<GaplessExtension> extend(const Graph& g, const gb_scores& scores,
                                      const std::vector<std::pair<uint32_t, int64_t>>& cluster,
                                      std::string sequence, size_t max_mismatches,
-                                     double overlap_threshold, bool trim);
+                                     double overlap_threshold, bool trim, ExtendTrace* trace = nullptr);
 
 // ---- LazyRNG, utility.cpp:907-931 / utility.hpp:698-794 -------------------------------
 class LazyRNG {

@@ -22,6 +22,21 @@ int oracle_extend(const gb_flat_index* ix, const gb_scores* scores,
                   uint32_t* path_pool, uint32_t path_cap,
                   uint32_t* mism_pool, uint32_t mism_cap);
 
+/* The GB_ITEM_* status gb_extend_batch gives the same call when its warp has a q_cap-entry frontier and an
+ * a_cap-node path arena (extend.cuh: EXTEND_Q_CAP, EXTEND_A_CAP) and the item has max_ext / path_cap / mism_cap output
+ * strides.  Each capacity is checked where the kernel checks it (frontier and arena before every push of the search,
+ * records and path nodes when a seed's best match is added, the mismatch pool after the full-length or duplicate
+ * filter, before trimming); the first one exceeded decides.  needs_out[5] (may be NULL): raw records, raw path nodes,
+ * pre-trim mismatches, peak frontier entries, peak arena nodes of one seed.  seed_skip[n_seeds] (may be NULL):
+ * 0 extended, 1 skipped because an exact full-length extension contains it, 2 skipped as invalid (see
+ * gb_extend_batch). */
+int oracle_extend_limits(const gb_flat_index* ix, const gb_scores* scores,
+                         const uint8_t* read, uint32_t read_len,
+                         const gb_seed* seeds, uint32_t n_seeds,
+                         uint32_t max_mismatches, double overlap_threshold, int trim,
+                         uint32_t q_cap, uint32_t a_cap, uint32_t max_ext, uint32_t path_cap, uint32_t mism_cap,
+                         uint64_t* needs_out, uint8_t* seed_skip);
+
 /* Haplotype-consistency primitives, exposed so tests can cross-check the flat GBWT
  * against brute-force path scanning.  state = {fwd_node,fwd_lo,fwd_hi,bwd_node,bwd_lo,bwd_hi}
  * (closed ranges as int64).  Returns number of successor states written (each 6 int64). */

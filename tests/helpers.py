@@ -24,6 +24,9 @@ def oracle_lib_configure(lib):
     lib.oracle_extend.argtypes = [C.POINTER(capi.FlatIndex), C.POINTER(capi.Scores), vp, u32, vp, u32, u32,
                                   C.c_double, C.c_int, vp, u32, vp, u32, vp, u32]
     lib.oracle_extend.restype = C.c_int
+    lib.oracle_extend_limits.argtypes = [C.POINTER(capi.FlatIndex), C.POINTER(capi.Scores), vp, u32, vp, u32, u32,
+                                         C.c_double, C.c_int, u32, u32, u32, u32, u32, vp, vp]
+    lib.oracle_extend_limits.restype = C.c_int
     lib.oracle_bd_state.argtypes = [C.POINTER(capi.FlatIndex), u32, vp]
     lib.oracle_bd_state.restype = C.c_int
     lib.oracle_follow_paths.argtypes = [C.POINTER(capi.FlatIndex), vp, C.c_int, vp, C.c_int]
@@ -70,6 +73,29 @@ def oracle_extend(index: capi.HostIndex, read, seeds, max_mismatches=4, overlap_
     return [expand_extension(ext[i], pp, mp) for i in range(n)]
 
 
+EXTEND_NEEDS = ("records", "path_nodes", "mismatches", "frontier", "arena")
+
+
+def oracle_extend_limits(index: capi.HostIndex, read, seeds, q_cap=0xFFFFFFFF, a_cap=0xFFFFFFFF, max_ext=0xFFFFFFFF,
+                         path_cap=0xFFFFFFFF, mism_cap=0xFFFFFFFF, max_mismatches=4, overlap_threshold=0.8, trim=True,
+                         scores=None):
+    """oracle_extend_limits: (GB_ITEM_* status under these capacities, needs dict keyed by EXTEND_NEEDS,
+    per-input-seed skip codes: 0 extended, 1 inside the exact full-length extension, 2 invalid)."""
+    lib = oracle_lib()
+    scores = scores or capi.DEFAULT_SCORES
+    rb = read.encode() if isinstance(read, str) else bytes(read)
+    rbuf = np.frombuffer(rb + b"\0", dtype=np.uint8).copy()
+    sd = np.zeros(max(1, len(seeds)), dtype=capi.seed_dt)
+    for i, (node, diag) in enumerate(seeds):
+        sd[i] = (node, diag)
+    needs = np.zeros(len(EXTEND_NEEDS), dtype=np.uint64)
+    skip = np.zeros(max(1, len(seeds)), dtype=np.uint8)
+    status = lib.oracle_extend_limits(C.byref(index.view), C.byref(scores), capi.ptr(rbuf), len(rb), capi.ptr(sd), len(seeds),
+                                      max_mismatches, overlap_threshold, 1 if trim else 0, q_cap, a_cap, max_ext, path_cap,
+                                      mism_cap, capi.ptr(needs), capi.ptr(skip))
+    return int(status), dict(zip(EXTEND_NEEDS, (int(x) for x in needs))), skip[:len(seeds)].tolist()
+
+
 def expand_extension(e, path_pool, mism_pool) -> dict:
     return {
         "path": [int(x) for x in path_pool[int(e["path_off"]): int(e["path_off"]) + int(e["path_len"])]],
@@ -77,15 +103,19 @@ def expand_extension(e, path_pool, mism_pool) -> dict:
         "offset": int(e["offset"]), "read_lo": int(e["read_lo"]), "read_hi": int(e["read_hi"]),
         "score": int(e["score"]), "left_full": bool(e["flags"] & 1), "right_full": bool(e["flags"] & 2),
         "state": tuple(int(e[f]) for f in ("fwd_node", "fwd_lo", "fwd_hi", "bwd_node", "bwd_lo", "bwd_hi")),
+        "mismatch_count": int(e["mismatches"]),
     }
 
 
-def gpu_extensions(ext_count, status, ext, path_pool, mism_pool, max_ext):
-    """Expand gb_extend_batch outputs into per-item lists of dict extensions."""
+def gpu_extensions(ext_count, status, ext, path_pool, mism_pool, max_ext, with_status=False):
+    """Expand gb_extend_batch outputs into per-item lists of dict extensions, every status asserted GB_ITEM_OK;
+    with_status=True returns per-item (status, extensions) instead, refused items included as they came back."""
     out = []
     for i in range(len(ext_count)):
-        assert status[i] == capi.GB_ITEM_OK, f"item {i} status {status[i]}"
-        out.append([expand_extension(ext[i * max_ext + j], path_pool, mism_pool) for j in range(int(ext_count[i]))])
+        if not with_status:
+            assert status[i] == capi.GB_ITEM_OK, f"item {i} status {status[i]}"
+        exts = [expand_extension(ext[i * max_ext + j], path_pool, mism_pool) for j in range(int(ext_count[i]))]
+        out.append((int(status[i]), exts) if with_status else exts)
     return out
 
 

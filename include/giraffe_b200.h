@@ -32,6 +32,15 @@ extern "C" {
 #define GB_ERR_CAPACITY      -4   /* an output capacity given by the caller was too small   */
 #define GB_ERR_FORMAT        -5   /* flat index failed validation                           */
 
+/* No C++ exception leaves an entry point that returns a status: one that escapes its body becomes a status code, and
+ * gb_last_error() says why.
+ *   out of host memory (std::bad_alloc)  GB_ERR_CAPACITY, "<entry point>: out of host memory"
+ *   any other exception                  GB_ERR_ARG, or GB_ERR_FORMAT from the readers of GBZ, .min and flat index files
+ *                                        (gb_index_from_gbz, gb_index_from_gbz_min, gb_index_load), with the
+ *                                        exception's message; the readers also set *out to NULL
+ * Entry points that return void or a pointer (gb_fragment_create, gb_fragment_register) have no status to report one
+ * with and are not covered. */
+
 /* per-item status byte */
 #define GB_ITEM_OK            0
 #define GB_ITEM_QUEUE_FULL    1   /* best-first frontier exceeded the per-warp workspace    */

@@ -132,117 +132,71 @@ def load_library() -> C.CDLL:
     if not path.exists():
         raise RuntimeError(f"{path} is missing: run `python -m vg_b200.build` (there is no fallback path)")
     lib = C.CDLL(str(path))
-    vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
-    lib.gb_index_build.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32, u32, C.POINTER(vp)]
-    lib.gb_index_build.restype = C.c_int
-    lib.gb_index_free.argtypes = [vp]
-    lib.gb_index_free.restype = None
-    lib.gb_index_view.argtypes = [vp, C.POINTER(FlatIndex)]
-    lib.gb_index_view.restype = C.c_int
-    lib.gb_device_create.argtypes = [C.POINTER(FlatIndex), C.c_int, C.POINTER(vp)]
-    lib.gb_device_create.restype = C.c_int
-    lib.gb_device_destroy.argtypes = [vp]
-    lib.gb_device_destroy.restype = None
-    lib.gb_last_error.argtypes = []
-    lib.gb_last_error.restype = C.c_char_p
-    lib.gb_index_from_gbz.argtypes = [C.c_char_p, u32, u32, vp]
-    lib.gb_index_from_gbz.restype = C.c_int
-    lib.gb_index_from_gbz_min.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, vp]
-    lib.gb_index_from_gbz_min.restype = C.c_int
-    lib.gb_index_build_with_hits.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32, u32, u64, vp, vp, vp]
-    lib.gb_index_build_with_hits.restype = C.c_int
-    lib.gb_index_build_from_gbwt.argtypes = [u32, vp, vp, u32, vp, u64, vp, vp, u32, u32, u64, vp, vp, vp]
-    lib.gb_index_build_from_gbwt.restype = C.c_int
-    lib.gb_index_save.argtypes = [C.POINTER(FlatIndex), C.c_char_p]
-    lib.gb_index_save.restype = C.c_int
-    lib.gb_index_load.argtypes = [C.c_char_p, vp]
-    lib.gb_index_load.restype = C.c_int
-    lib.gb_set_scores.argtypes = [vp, C.POINTER(Scores)]
-    lib.gb_set_scores.restype = C.c_int
-    lib.gb_extend_batch.argtypes = [vp, C.POINTER(ExtendParams), u32, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.gb_extend_batch.restype = C.c_int
-    lib.gb_map_params_default.argtypes = [C.POINTER(MapParams)]
-    lib.gb_map_params_default.restype = None
-    lib.gb_map_batch.argtypes = [vp, C.POINTER(MapParams), u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, vp, vp]
-    lib.gb_map_batch.restype = C.c_int
-    lib.gb_map_paired_batch.argtypes = [vp, C.POINTER(MapParams), u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, vp, vp]
-    lib.gb_map_batch_device.argtypes = [vp, C.POINTER(MapParams), C.c_int, u32, vp, vp, vp, u32, vp, vp, u64, vp, u64, vp, vp]
-    lib.gb_map_batch_device.restype = C.c_int
-    lib.gb_device_set_stream.argtypes = [vp, vp]
-    lib.gb_device_set_stream.restype = C.c_int
-    lib.gb_device_synchronize.argtypes = [vp]
-    lib.gb_device_synchronize.restype = C.c_int
-    lib.gb_stage_times.argtypes = [vp, vp]
-    lib.gb_stage_times.restype = C.c_int
-    lib.gb_map_paired_batch.restype = C.c_int
-    lib.gb_xdrop_pinned_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp]
-    lib.gb_xdrop_pinned_batch.restype = C.c_int
-    lib.gb_sw_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp]
-    lib.gb_sw_batch.restype = C.c_int
-    lib.gb_banded_global_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp]
-    lib.gb_banded_global_batch.restype = C.c_int
-    lib.gb_xdrop_dag_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp]
-    lib.gb_xdrop_dag_batch.restype = C.c_int
-    lib.gb_wfa_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.gb_wfa_batch.restype = C.c_int
-    lib.gb_chain_params_default.argtypes = [C.POINTER(ChainParams)]
-    lib.gb_chain_params_default.restype = None
-    lib.gb_chain_batch.argtypes = [vp, C.POINTER(ChainParams), u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.gb_chain_batch.restype = C.c_int
-    lib.gb_chain_batch_transitions.argtypes = [vp, C.POINTER(ChainParams), u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.gb_chain_batch_transitions.restype = C.c_int
-    lib.gb_chain_anchors.argtypes = [C.POINTER(FlatIndex), C.POINTER(Scores), u32, vp, vp, vp, vp, vp, vp]
-    lib.gb_chain_anchors.restype = C.c_int
-    lib.gb_chain_candidates_batch.argtypes = [vp, u32, vp, vp, u64, vp, u64, vp]
-    lib.gb_chain_candidates_batch.restype = C.c_int
-    lib.gb_fragment_create.argtypes = [u64, u64, C.c_double]
-    lib.gb_fragment_create.restype = vp
-    lib.gb_fragment_destroy.argtypes = [vp]
-    lib.gb_fragment_destroy.restype = None
-    lib.gb_fragment_force.argtypes = [vp, C.c_double, C.c_double]
-    lib.gb_fragment_force.restype = None
-    lib.gb_fragment_register.argtypes = [vp, C.c_int64]
-    lib.gb_fragment_register.restype = None
-    lib.gb_fragment_finalize.argtypes = [vp]
-    lib.gb_fragment_finalize.restype = None
-    lib.gb_fragment_mean.argtypes = [vp]
-    lib.gb_fragment_mean.restype = C.c_double
-    lib.gb_fragment_stdev.argtypes = [vp]
-    lib.gb_fragment_stdev.restype = C.c_double
-    lib.gb_fragment_is_finalized.argtypes = [vp]
-    lib.gb_fragment_is_finalized.restype = C.c_int
-    lib.gb_fragment_sample_size.argtypes = [vp]
-    lib.gb_fragment_sample_size.restype = u64
-    lib.gb_map_paired_job.argtypes = [vp, C.POINTER(MapParams), vp, u32, u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, vp, vp, vp]
-    lib.gb_map_paired_job.restype = C.c_int
-    for fn in (lib.gb_emit_gaf, lib.gb_emit_json, lib.gb_emit_gam):
-        fn.argtypes = [C.POINTER(FlatIndex), u32, vp, vp, u64, vp, u64, u32, vp, vp, vp, vp, vp, vp, u64, vp]
-        fn.restype = C.c_int
-    for fn in (lib.gb_emit_gaf_device, lib.gb_emit_gam_device):
-        fn.argtypes = [vp, u32, vp, vp, u64, vp, u64, u32, vp, vp, vp, vp, vp, vp, u64, vp]
-        fn.restype = C.c_int
-    lib.gb_debug_seed_stage.argtypes = [vp, C.POINTER(MapParams), C.c_int, u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, u64]
-    lib.gb_debug_seed_stage.restype = C.c_int
-    lib.gb_device_pool_overflow.argtypes = [vp, C.POINTER(C.c_int)]
-    lib.gb_device_pool_overflow.restype = C.c_int
-    lib.gb_kernel_times.argtypes = [vp, u32, vp, vp, vp]
-    lib.gb_kernel_times.restype = C.c_int
-    lib.gb_device_set_output_mirror.argtypes = [vp, vp, vp, u64, vp, u64]
-    lib.gb_device_set_output_mirror.restype = C.c_int
-    lib.gb_plan_stats.argtypes = [vp, vp]
-    lib.gb_plan_stats.restype = C.c_int
-    lib.gb_bgzf_compress.argtypes = [vp, u64, C.c_int, vp, u64, vp]
-    lib.gb_bgzf_compress.restype = C.c_int
-    lib.gb_bgzf_compress_device.argtypes = [vp, vp, u64, vp, u64, vp]
-    lib.gb_bgzf_compress_device.restype = C.c_int
-    lib.gb_bgzf_decompress_device.argtypes = [vp, vp, u64, C.c_int, vp, u64, vp, vp]
-    lib.gb_bgzf_decompress_device.restype = C.c_int
-    lib.gb_fastq_parse_device.argtypes = [vp, u32, vp, vp, u32, C.c_int, u32, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp]
-    lib.gb_fastq_parse_device.restype = C.c_int
-    lib.gb_last_kernel_ms.argtypes = [vp]
-    lib.gb_last_kernel_ms.restype = C.c_float
-    lib.gb_launch_count.argtypes = [vp]
-    lib.gb_launch_count.restype = C.c_uint64
+    vp, u32, u64, st, fix = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int, C.POINTER(FlatIndex)
+    emit = [u32, vp, vp, u64, vp, u64, u32, vp, vp, vp, vp, vp, vp, u64, vp]      # gb_emit_* after the index / device
+    seam_out = [vp, vp, vp, vp, vp, vp]                                            # score, maps, edits, n_maps, n_edits, status
+    signatures = {                                                                 # name: (restype, argtypes)
+        "gb_index_build": (st, [u32, vp, vp, u32, vp, vp, vp, u32, u32, C.POINTER(vp)]),
+        "gb_index_free": (None, [vp]),
+        "gb_index_view": (st, [vp, fix]),
+        "gb_device_create": (st, [fix, C.c_int, C.POINTER(vp)]),
+        "gb_device_destroy": (None, [vp]),
+        "gb_last_error": (C.c_char_p, []),
+        "gb_index_from_gbz": (st, [C.c_char_p, u32, u32, vp]),
+        "gb_index_from_gbz_min": (st, [C.c_char_p, C.c_char_p, C.c_char_p, vp]),
+        "gb_index_build_with_hits": (st, [u32, vp, vp, u32, vp, vp, vp, u32, u32, u64, vp, vp, vp]),
+        "gb_index_build_from_gbwt": (st, [u32, vp, vp, u32, vp, u64, vp, vp, u32, u32, u64, vp, vp, vp]),
+        "gb_index_save": (st, [fix, C.c_char_p]),
+        "gb_index_load": (st, [C.c_char_p, vp]),
+        "gb_set_scores": (st, [vp, C.POINTER(Scores)]),
+        "gb_extend_batch": (st, [vp, C.POINTER(ExtendParams), u32, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "gb_map_params_default": (None, [C.POINTER(MapParams)]),
+        "gb_map_batch": (st, [vp, C.POINTER(MapParams), u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, vp, vp]),
+        "gb_map_paired_batch": (st, [vp, C.POINTER(MapParams), u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, vp, vp]),
+        "gb_map_batch_device": (st, [vp, C.POINTER(MapParams), C.c_int, u32, vp, vp, vp, u32, vp, vp, u64, vp, u64, vp, vp]),
+        "gb_device_set_stream": (st, [vp, vp]),
+        "gb_device_synchronize": (st, [vp]),
+        "gb_stage_times": (st, [vp, vp]),
+        "gb_xdrop_pinned_batch": (st, [vp, u32, vp, vp, vp, vp, vp, vp, vp, u32, u32, *seam_out]),
+        "gb_sw_batch": (st, [vp, u32, vp, vp, vp, vp, vp, vp, u32, u32, *seam_out]),
+        "gb_banded_global_batch": (st, [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, *seam_out]),
+        "gb_xdrop_dag_batch": (st, [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, *seam_out]),
+        "gb_wfa_batch": (st, [vp, u32, vp, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "gb_chain_params_default": (None, [C.POINTER(ChainParams)]),
+        "gb_chain_batch": (st, [vp, C.POINTER(ChainParams), u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "gb_chain_batch_transitions": (st, [vp, C.POINTER(ChainParams), u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "gb_chain_anchors": (st, [fix, C.POINTER(Scores), u32, vp, vp, vp, vp, vp, vp]),
+        "gb_chain_candidates_batch": (st, [vp, u32, vp, vp, u64, vp, u64, vp]),
+        "gb_fragment_create": (vp, [u64, u64, C.c_double]),
+        "gb_fragment_destroy": (None, [vp]),
+        "gb_fragment_force": (None, [vp, C.c_double, C.c_double]),
+        "gb_fragment_register": (None, [vp, C.c_int64]),
+        "gb_fragment_finalize": (None, [vp]),
+        "gb_fragment_mean": (C.c_double, [vp]),
+        "gb_fragment_stdev": (C.c_double, [vp]),
+        "gb_fragment_is_finalized": (st, [vp]),
+        "gb_fragment_sample_size": (u64, [vp]),
+        "gb_map_paired_job": (st, [vp, C.POINTER(MapParams), vp, u32, u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, vp, vp, vp]),
+        "gb_emit_gaf": (st, [fix, *emit]),
+        "gb_emit_json": (st, [fix, *emit]),
+        "gb_emit_gam": (st, [fix, *emit]),
+        "gb_emit_gaf_device": (st, [vp, *emit]),
+        "gb_emit_gam_device": (st, [vp, *emit]),
+        "gb_debug_seed_stage": (st, [vp, C.POINTER(MapParams), C.c_int, u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, u64]),
+        "gb_device_pool_overflow": (st, [vp, C.POINTER(C.c_int)]),
+        "gb_kernel_times": (st, [vp, u32, vp, vp, vp]),
+        "gb_device_set_output_mirror": (st, [vp, vp, vp, u64, vp, u64]),
+        "gb_plan_stats": (st, [vp, vp]),
+        "gb_bgzf_compress": (st, [vp, u64, C.c_int, vp, u64, vp]),
+        "gb_bgzf_compress_device": (st, [vp, vp, u64, vp, u64, vp]),
+        "gb_bgzf_decompress_device": (st, [vp, vp, u64, C.c_int, vp, u64, vp, vp]),
+        "gb_fastq_parse_device": (st, [vp, u32, vp, vp, u32, C.c_int, u32, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp]),
+        "gb_last_kernel_ms": (C.c_float, [vp]),
+        "gb_launch_count": (u64, [vp]),
+    }
+    for name, (restype, argtypes) in signatures.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 
@@ -309,6 +263,21 @@ class GbError(RuntimeError):
         self.code = code
 
 
+def _check(rc: int, what: str) -> None:
+    if rc != GB_OK:
+        raise GbError(rc, what)
+
+
+def _retry_on_capacity(call, out, grow):
+    """rc = call(out); when rc is GB_ERR_CAPACITY and grow is given, call once more with out = grow(), sized from what the
+    first call reported.  Returns (rc, the out of the last call)."""
+    rc = call(out)
+    if rc == GB_ERR_CAPACITY and grow is not None:
+        out = grow()
+        rc = call(out)
+    return rc, out
+
+
 class HostIndex:
     """Owns a gb_host_index built by the library from node sequences and haplotype paths."""
 
@@ -336,40 +305,29 @@ class HostIndex:
             assert len(hk) == len(hp)
             rc = lib.gb_index_build_with_hits(n, ptr(seq), ptr(node_off), len(paths), ptr(flat), ptr(path_off), dptr, k, w,
                                               len(hk), ptr(hk), ptr(hp), C.byref(h))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_build")
+        _check(rc, "gb_index_build")
+        self._adopt(h, list(node_seqs), [list(p) for p in paths], k, w)
+
+    def _adopt(self, h, node_seqs, paths, k=None, w=None):
+        """Take ownership of the gb_host_index h and view it; k and w default to the index's own."""
         self._h = h
         self.view = FlatIndex()
-        rc = lib.gb_index_view(h, C.byref(self.view))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_view")
-        self.node_seqs = list(node_seqs)
-        self.paths = [list(p) for p in paths]
-        self.k, self.w = k, w
+        _check(load_library().gb_index_view(h, C.byref(self.view)), "gb_index_view")
+        self.node_seqs, self.paths = node_seqs, paths
+        self.k, self.w = (int(self.view.k), int(self.view.w)) if k is None else (k, w)
+        return self
 
     def save(self, path):
         """gb_index_save: the flat index as one file."""
-        rc = load_library().gb_index_save(C.byref(self.view), str(path).encode())
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_save")
+        _check(load_library().gb_index_save(C.byref(self.view), str(path).encode()), "gb_index_save")
 
     @classmethod
     def from_gbz(cls, path, k=29, w=11):
         """gb_index_from_gbz: the flat index of a GBZ file (graphs that are chains of bubbles)."""
         lib = load_library()
         h = C.c_void_p()
-        rc = lib.gb_index_from_gbz(str(path).encode(), k, w, C.byref(h))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_from_gbz")
-        self = cls.__new__(cls)
-        self._h = h
-        self.view = FlatIndex()
-        rc = lib.gb_index_view(h, C.byref(self.view))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_view")
-        self.node_seqs, self.paths = None, None
-        self.k, self.w = k, w
-        return self
+        _check(lib.gb_index_from_gbz(str(path).encode(), k, w, C.byref(h)), "gb_index_from_gbz")
+        return cls.__new__(cls)._adopt(h, None, None, k, w)
 
     @classmethod
     def from_gbwt(cls, node_seqs, n_paths, gbwt_words, rec_off, dist=None, k=29, w=11, hits=None):
@@ -387,55 +345,27 @@ class HostIndex:
         if hits is not None:
             hk, hp = (np.ascontiguousarray(a, dtype=np.uint64) for a in hits)
         h = C.c_void_p()
-        rc = lib.gb_index_build_from_gbwt(n, ptr(seq), ptr(node_off), n_paths, ptr(words), len(words), ptr(ro), dptr, k, w,
-                                          0 if hk is None else len(hk), None if hk is None else ptr(hk), None if hp is None else ptr(hp), C.byref(h))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_build_from_gbwt")
-        self = cls.__new__(cls)
-        self._h = h
-        self.view = FlatIndex()
-        rc = lib.gb_index_view(h, C.byref(self.view))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_view")
-        self.node_seqs, self.paths = list(node_seqs), None
-        self.k, self.w = k, w
-        return self
+        _check(lib.gb_index_build_from_gbwt(n, ptr(seq), ptr(node_off), n_paths, ptr(words), len(words), ptr(ro), dptr, k, w,
+                                            0 if hk is None else len(hk), None if hk is None else ptr(hk), None if hp is None else ptr(hp),
+                                            C.byref(h)), "gb_index_build_from_gbwt")
+        return cls.__new__(cls)._adopt(h, list(node_seqs), None, k, w)
 
     @classmethod
     def from_gbz_min(cls, gbz, min_path, zipcodes=None):
         """gb_index_from_gbz_min: GBZ + the .min (and .zipcodes) files giraffe loads beside it; k and w come from the .min."""
         lib = load_library()
         h = C.c_void_p()
-        rc = lib.gb_index_from_gbz_min(str(gbz).encode(), str(min_path).encode(), str(zipcodes).encode() if zipcodes else None, C.byref(h))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_from_gbz_min")
-        self = cls.__new__(cls)
-        self._h = h
-        self.view = FlatIndex()
-        rc = lib.gb_index_view(h, C.byref(self.view))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_view")
-        self.node_seqs, self.paths = None, None
-        self.k, self.w = int(self.view.k), int(self.view.w)
-        return self
+        _check(lib.gb_index_from_gbz_min(str(gbz).encode(), str(min_path).encode(), str(zipcodes).encode() if zipcodes else None,
+                                         C.byref(h)), "gb_index_from_gbz_min")
+        return cls.__new__(cls)._adopt(h, None, None)
 
     @classmethod
     def load(cls, path):
         """gb_index_load: an index written by save()."""
         lib = load_library()
         h = C.c_void_p()
-        rc = lib.gb_index_load(str(path).encode(), C.byref(h))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_load")
-        self = cls.__new__(cls)
-        self._h = h
-        self.view = FlatIndex()
-        rc = lib.gb_index_view(h, C.byref(self.view))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_index_view")
-        self.node_seqs, self.paths = None, None
-        self.k, self.w = int(self.view.k), int(self.view.w)
-        return self
+        _check(lib.gb_index_load(str(path).encode(), C.byref(h)), "gb_index_load")
+        return cls.__new__(cls)._adopt(h, None, None)
 
     def array(self, name: str) -> np.ndarray:
         v = self.view
@@ -477,9 +407,8 @@ def chain_anchors(index, seeds, min_offset, min_is_reverse, min_length, paths=No
     pa = None if paths is None else np.ascontiguousarray(list(paths) + [0], dtype=np.uint64)
     out = np.zeros(n + 1, dtype=chain_anchor_dt)
     sc = scores or DEFAULT_SCORES
-    rc = lib.gb_chain_anchors(C.byref(index.view), C.byref(sc), n, ptr(pos), ptr(mo), ptr(mr), ptr(ml), None if pa is None else ptr(pa), ptr(out))
-    if rc != GB_OK:
-        raise GbError(rc, "gb_chain_anchors")
+    _check(lib.gb_chain_anchors(C.byref(index.view), C.byref(sc), n, ptr(pos), ptr(mo), ptr(mr), ptr(ml), None if pa is None else ptr(pa),
+                                ptr(out)), "gb_chain_anchors")
     return out[:n]
 
 
@@ -498,11 +427,9 @@ def emit_text(kind, flat_index, aln, maps, edits, rbuf, qbuf, read_off, names=No
     cap = 4096 + len(aln) * 4096
     out = np.zeros(cap, dtype=np.uint8)
     used = C.c_uint64()
-    rc = fn(C.byref(flat_index), len(aln), ptr(aln), ptr(maps), len(maps), ptr(edits), len(edits), len(read_off) - 1, ptr(rbuf),
-            ptr(qbuf) if qbuf is not None else None, ptr(read_off), ptr(nbuf) if nbuf is not None else None, ptr(noff) if noff is not None else None,
-            ptr(out), cap, C.byref(used))
-    if rc != GB_OK:
-        raise GbError(rc, "gb_emit_" + kind)
+    _check(fn(C.byref(flat_index), len(aln), ptr(aln), ptr(maps), len(maps), ptr(edits), len(edits), len(read_off) - 1, ptr(rbuf),
+              ptr(qbuf) if qbuf is not None else None, ptr(read_off), ptr(nbuf) if nbuf is not None else None, ptr(noff) if noff is not None else None,
+              ptr(out), cap, C.byref(used)), "gb_emit_" + kind)
     data = out[: used.value].tobytes()
     return data if kind == "gam" else data.decode()
 
@@ -526,9 +453,7 @@ def bgzf_compress(data: bytes, level: int = 6) -> bytes:
     cap = len(data) + 128 * (len(data) // 0xff00 + 2)
     out = np.zeros(cap, dtype=np.uint8)
     used = C.c_uint64()
-    rc = lib.gb_bgzf_compress(ptr(src), len(data), level, ptr(out), cap, C.byref(used))
-    if rc != GB_OK:
-        raise GbError(rc, "gb_bgzf_compress")
+    _check(lib.gb_bgzf_compress(ptr(src), len(data), level, ptr(out), cap, C.byref(used)), "gb_bgzf_compress")
     return out[: used.value].tobytes()
 
 
@@ -586,9 +511,7 @@ class Device:
     def __init__(self, index: HostIndex, ordinal: int = 0, scores: Scores | None = None):
         lib = load_library()
         h = C.c_void_p()
-        rc = lib.gb_device_create(C.byref(index.view), ordinal, C.byref(h))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_device_create")
+        _check(lib.gb_device_create(C.byref(index.view), ordinal, C.byref(h)), "gb_device_create")
         self._h = h
         self.index = index
         if scores is not None:
@@ -637,11 +560,9 @@ class Device:
         ext = np.zeros(n_items * max_ext, dtype=extension_dt)
         path_pool = np.zeros(n_items * path_cap, dtype=np.uint32)
         mism_pool = np.zeros(n_items * mism_cap, dtype=np.uint32)
-        rc = lib.gb_extend_batch(self._h, C.byref(p), len(read_off) - 1, ptr(rbuf), ptr(read_off), n_items,
-                                 ptr(item_read), ptr(seeds), ptr(seed_off), ptr(ext_count), ptr(status), ptr(ext),
-                                 ptr(path_pool), ptr(mism_pool))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_extend_batch")
+        _check(lib.gb_extend_batch(self._h, C.byref(p), len(read_off) - 1, ptr(rbuf), ptr(read_off), n_items,
+                                   ptr(item_read), ptr(seeds), ptr(seed_off), ptr(ext_count), ptr(status), ptr(ext),
+                                   ptr(path_pool), ptr(mism_pool)), "gb_extend_batch")
         return ext_count, status, ext, path_pool, mism_pool
 
     def xdrop_pinned_batch(self, problems, map_cap=256, edit_cap=1024, with_status=False):
@@ -661,10 +582,8 @@ class Device:
         q = np.frombuffer(b"".join(bytes(p[3]) for p in problems) + b"\0", dtype=np.uint8).copy()
         gap = np.array([p[4] for p in problems], dtype=np.uint32)
         score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
-        rc = lib.gb_xdrop_pinned_batch(self._h, n, ptr(par), ptr(nodes), ptr(tree_off), ptr(trim), ptr(q), ptr(query_off),
-                                       ptr(gap), map_cap, edit_cap, *map(ptr, outs))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_xdrop_pinned_batch")
+        _check(lib.gb_xdrop_pinned_batch(self._h, n, ptr(par), ptr(nodes), ptr(tree_off), ptr(trim), ptr(q), ptr(query_off),
+                                         ptr(gap), map_cap, edit_cap, *map(ptr, outs)), "gb_xdrop_pinned_batch")
         if with_status:
             return [(int(status[i]), int(score[i]),
                      decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i], node_offset=1) if status[i] == GB_ITEM_OK else [])
@@ -685,9 +604,7 @@ class Device:
         n = len(problems)
         dags = _pack_dags(problems)
         outs = _seam_outputs(n, map_cap, edit_cap)
-        rc = lib.gb_sw_batch(self._h, n, *map(ptr, dags), map_cap, edit_cap, *map(ptr, outs))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_sw_batch")
+        _check(lib.gb_sw_batch(self._h, n, *map(ptr, dags), map_cap, edit_cap, *map(ptr, outs)), "gb_sw_batch")
         return _dag_seam_results(outs, map_cap, with_status)
 
     def banded_global_batch(self, problems, map_cap=512, edit_cap=2048):
@@ -700,10 +617,8 @@ class Device:
         permissive = np.asarray([1 if p[4] else 0 for p in problems], dtype=np.uint8)
         dags = _pack_dags(problems)
         score, maps, edits, nm, _, status = outs = _seam_outputs(n, map_cap, edit_cap)
-        rc = lib.gb_banded_global_batch(self._h, n, *map(ptr, dags), ptr(pad), ptr(permissive), map_cap, edit_cap,
-                                        *map(ptr, outs))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_banded_global_batch")
+        _check(lib.gb_banded_global_batch(self._h, n, *map(ptr, dags), ptr(pad), ptr(permissive), map_cap, edit_cap,
+                                          *map(ptr, outs)), "gb_banded_global_batch")
         return [(int(status[i]), int(score[i]), decode_path(maps[i * map_cap:], edits[i * edit_cap:], nm[i])) for i in range(n)]
 
     def xdrop_dag_batch(self, problems, map_cap=512, edit_cap=2048, with_status=False):
@@ -716,10 +631,8 @@ class Device:
         gap = np.array([p[4] for p in problems], dtype=np.uint32)
         dags = _pack_dags(problems)
         outs = _seam_outputs(n, map_cap, edit_cap)
-        rc = lib.gb_xdrop_dag_batch(self._h, n, *map(ptr, dags), ptr(seed), ptr(gap), map_cap, edit_cap,
-                                    *map(ptr, outs))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_xdrop_dag_batch")
+        _check(lib.gb_xdrop_dag_batch(self._h, n, *map(ptr, dags), ptr(seed), ptr(gap), map_cap, edit_cap,
+                                      *map(ptr, outs)), "gb_xdrop_dag_batch")
         return _dag_seam_results(outs, map_cap, with_status)
 
     def chain_candidates_batch(self, problems, limit=2 ** 64 - 1, cap=None):
@@ -732,13 +645,11 @@ class Device:
         coff = np.zeros(n + 1, dtype=np.uint64)
         if cap is None:
             rc = lib.gb_chain_candidates_batch(self._h, n, ptr(pos), ptr(off), limit, None, 0, ptr(coff))      # sizes first
-            if rc not in (GB_OK, GB_ERR_CAPACITY):
-                raise GbError(rc, "gb_chain_candidates_batch")
+            if rc != GB_ERR_CAPACITY:
+                _check(rc, "gb_chain_candidates_batch")
             cap = int(coff[n])
         out = np.zeros(cap + 1, dtype=chain_candidate_dt)
-        rc = lib.gb_chain_candidates_batch(self._h, n, ptr(pos), ptr(off), limit, ptr(out), cap, ptr(coff))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_chain_candidates_batch")
+        _check(lib.gb_chain_candidates_batch(self._h, n, ptr(pos), ptr(off), limit, ptr(out), cap, ptr(coff)), "gb_chain_candidates_batch")
         return [out[int(coff[p]): int(coff[p + 1])].copy() for p in range(n)]
 
     def chain_batch(self, problems, params=None, transitions=False):
@@ -764,8 +675,7 @@ class Device:
         else:
             rc = lib.gb_chain_batch(self._h, C.byref(params), n, ptr(anchors), ptr(aoff), ptr(cands), ptr(coff),
                                     ptr(dps), ptr(dpsrc), ptr(dpp), ptr(dpr), ptr(nch), ptr(cs), ptr(cb), ptr(cc), ptr(items))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_chain_batch")
+        _check(rc, "gb_chain_batch")
         out = []
         for p in range(n):
             a0, a1 = int(aoff[p]), int(aoff[p + 1])
@@ -794,10 +704,8 @@ class Device:
         ok = np.zeros(n, dtype=np.int32); score = np.zeros(n, dtype=np.int32)
         noff, soff, length, npath, nedits = (np.zeros(n, dtype=np.uint32) for _ in range(5))
         path = np.zeros(n * path_cap, dtype=np.uint32); edits = np.zeros(n * edit_cap, dtype=np.uint32)
-        rc = lib.gb_wfa_batch(self._h, n, ptr(seq), ptr(seq_off), ptr(mode), ptr(pos), None if em is None else ptr(em), path_cap, edit_cap,
-                              ptr(ok), ptr(score), ptr(noff), ptr(soff), ptr(length), ptr(path), ptr(npath), ptr(edits), ptr(nedits))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_wfa_batch")
+        _check(lib.gb_wfa_batch(self._h, n, ptr(seq), ptr(seq_off), ptr(mode), ptr(pos), None if em is None else ptr(em), path_cap, edit_cap,
+                                ptr(ok), ptr(score), ptr(noff), ptr(soff), ptr(length), ptr(path), ptr(npath), ptr(edits), ptr(nedits)), "gb_wfa_batch")
         out = []
         for i in range(n):
             assert with_status or ok[i] >= 0, f"problem {i}: workspace capacity exceeded"
@@ -822,15 +730,13 @@ class Device:
             aln, maps, edits, status = out
         used = (C.c_uint64(), C.c_uint64())
         fn = lib.gb_map_paired_batch if paired else lib.gb_map_batch
-        rc = fn(self._h, C.byref(p), n, ptr(rbuf), ptr(qbuf) if qbuf is not None else None, ptr(read_off), ptr(aln),
-                ptr(maps), len(maps), ptr(edits), len(edits), ptr(status), C.byref(used[0]), C.byref(used[1]))
-        if rc == GB_ERR_CAPACITY and out is None:
-            maps = np.zeros(n * k * p.mapping_cap_per_read, dtype=mapping_dt)
-            edits = np.zeros(n * k * p.edit_cap_per_read, dtype=np.uint32)
-            rc = fn(self._h, C.byref(p), n, ptr(rbuf), ptr(qbuf) if qbuf is not None else None, ptr(read_off), ptr(aln),
-                    ptr(maps), len(maps), ptr(edits), len(edits), ptr(status), C.byref(used[0]), C.byref(used[1]))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_map_paired_batch" if paired else "gb_map_batch")
+        grow = None if out is not None else lambda: (np.zeros(n * k * p.mapping_cap_per_read, dtype=mapping_dt),
+                                                     np.zeros(n * k * p.edit_cap_per_read, dtype=np.uint32))
+        rc, (maps, edits) = _retry_on_capacity(
+            lambda me: fn(self._h, C.byref(p), n, ptr(rbuf), ptr(qbuf) if qbuf is not None else None, ptr(read_off), ptr(aln),
+                          ptr(me[0]), len(me[0]), ptr(me[1]), len(me[1]), ptr(status), C.byref(used[0]), C.byref(used[1])),
+            (maps, edits), grow)
+        _check(rc, "gb_map_paired_batch" if paired else "gb_map_batch")
         self.last_used = (used[0].value, used[1].value)
         return aln, maps, edits, status
 
@@ -846,11 +752,9 @@ class Device:
         status = np.zeros(n, dtype=np.uint8)
         route = np.zeros(n // 2, dtype=np.uint8)
         used = (C.c_uint64(), C.c_uint64())
-        rc = lib.gb_map_paired_job(self._h, C.byref(p), distribution._h, training_window, n, ptr(rbuf), ptr(qbuf) if qbuf is not None else None,
-                                   ptr(read_off), ptr(aln), ptr(maps), len(maps), ptr(edits), len(edits), ptr(status), ptr(route),
-                                   C.byref(used[0]), C.byref(used[1]))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_map_paired_job")
+        _check(lib.gb_map_paired_job(self._h, C.byref(p), distribution._h, training_window, n, ptr(rbuf), ptr(qbuf) if qbuf is not None else None,
+                                     ptr(read_off), ptr(aln), ptr(maps), len(maps), ptr(edits), len(edits), ptr(status), ptr(route),
+                                     C.byref(used[0]), C.byref(used[1])), "gb_map_paired_job")
         self.last_used = (used[0].value, used[1].value)
         return aln, maps, edits, status, route
 
@@ -860,41 +764,31 @@ class Device:
         p = params or default_map_params()
         n = len(read_off) - 1
         outs = stage_buffers(n, per_read)
-        rc = lib.gb_debug_seed_stage(self._h, C.byref(p), 1 if paired else 0, n, ptr(rbuf), ptr(qbuf) if qbuf is not None else None, ptr(read_off),
-                                     ptr(outs[0]), ptr(outs[1]), len(outs[1]), ptr(outs[2]), len(outs[2]), ptr(outs[3]), len(outs[3]),
-                                     ptr(outs[4]), len(outs[4]), ptr(outs[5]), len(outs[5]))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_debug_seed_stage")
+        _check(lib.gb_debug_seed_stage(self._h, C.byref(p), 1 if paired else 0, n, ptr(rbuf), ptr(qbuf) if qbuf is not None else None, ptr(read_off),
+                                       ptr(outs[0]), ptr(outs[1]), len(outs[1]), ptr(outs[2]), len(outs[2]), ptr(outs[3]), len(outs[3]),
+                                       ptr(outs[4]), len(outs[4]), ptr(outs[5]), len(outs[5])), "gb_debug_seed_stage")
         return outs
 
     def pool_overflow(self) -> bool:
         flag = C.c_int()
-        rc = load_library().gb_device_pool_overflow(self._h, C.byref(flag))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_device_pool_overflow")
+        _check(load_library().gb_device_pool_overflow(self._h, C.byref(flag)), "gb_device_pool_overflow")
         return bool(flag.value)
 
     def kernel_times(self):
         """Per-kernel device time of the last mapping call's last chunk: list of (kernel name, ms)."""
         cap = 48
         names = C.create_string_buffer(cap * 48); ms = (C.c_float * cap)(); n = C.c_uint32()
-        rc = load_library().gb_kernel_times(self._h, cap, names, ms, C.byref(n))
-        if rc != GB_OK:
-            raise GbError(rc, "gb_kernel_times")
+        _check(load_library().gb_kernel_times(self._h, cap, names, ms, C.byref(n)), "gb_kernel_times")
         return [(names.raw[i * 48:(i + 1) * 48].split(b"\0")[0].decode(), float(ms[i])) for i in range(n.value)]
 
     def plan_stats(self):
         out = (C.c_uint64 * 4)()
-        rc = load_library().gb_plan_stats(self._h, out)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_plan_stats")
+        _check(load_library().gb_plan_stats(self._h, out), "gb_plan_stats")
         return {"tails": int(out[0]), "trees": int(out[1]), "in_place": int(out[2]), "cells": int(out[3])}
 
     def stage_times(self):
         ms = (C.c_float * 4)()
-        rc = load_library().gb_stage_times(self._h, ms)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_stage_times")
+        _check(load_library().gb_stage_times(self._h, ms), "gb_stage_times")
         return [float(x) for x in ms]
 
     def emit_device(self, kind, aln, maps, edits, reads, read_off, quals=None, names=None, name_off=None, out=None):
@@ -913,17 +807,12 @@ class Device:
         if out is None:
             out = torch.empty(1, dtype=torch.uint8, device=reads.device)
         used = C.c_uint64()
-        for attempt in range(2):
-            rc = fn(self._h, n, vp(aln), vp(maps), n_maps, vp(edits), n_edits, read_off.numel() - 1, vp(reads), vp(quals), vp(read_off),
-                    vp(names), vp(name_off), vp(out), out.numel(), C.byref(used))
-            if rc != GB_ERR_CAPACITY or attempt:
-                break
-            out = torch.empty(max(1, used.value), dtype=torch.uint8, device=reads.device)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_emit_" + kind + "_device")
-        rc = lib.gb_device_synchronize(self._h)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_device_synchronize")
+        rc, out = _retry_on_capacity(
+            lambda o: fn(self._h, n, vp(aln), vp(maps), n_maps, vp(edits), n_edits, read_off.numel() - 1, vp(reads), vp(quals), vp(read_off),
+                         vp(names), vp(name_off), vp(o), o.numel(), C.byref(used)),
+            out, lambda: torch.empty(max(1, used.value), dtype=torch.uint8, device=reads.device))
+        _check(rc, "gb_emit_" + kind + "_device")
+        _check(lib.gb_device_synchronize(self._h), "gb_device_synchronize")
         return out[: used.value]
 
     def bgzf_compress_device(self, data, out=None):
@@ -937,17 +826,12 @@ class Device:
         if out is None:
             out = torch.empty(1, dtype=torch.uint8, device=data.device)
         used = C.c_uint64()
-        for attempt in range(2):
-            rc = lib.gb_bgzf_compress_device(self._h, C.c_void_p(data.data_ptr()) if data.numel() else None, data.numel(),
-                                             C.c_void_p(out.data_ptr()), out.numel(), C.byref(used))
-            if rc != GB_ERR_CAPACITY or attempt:
-                break
-            out = torch.empty(used.value, dtype=torch.uint8, device=data.device)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_bgzf_compress_device")
-        rc = lib.gb_device_synchronize(self._h)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_device_synchronize")
+        rc, out = _retry_on_capacity(
+            lambda o: lib.gb_bgzf_compress_device(self._h, C.c_void_p(data.data_ptr()) if data.numel() else None, data.numel(),
+                                                  C.c_void_p(o.data_ptr()), o.numel(), C.byref(used)),
+            out, lambda: torch.empty(used.value, dtype=torch.uint8, device=data.device))
+        _check(rc, "gb_bgzf_compress_device")
+        _check(lib.gb_device_synchronize(self._h), "gb_device_synchronize")
         return out[: used.value]
 
     def bgzf_decompress_device(self, data, final=True, out=None):
@@ -961,15 +845,11 @@ class Device:
         if out is None:
             out = torch.empty(1, dtype=torch.uint8, device=data.device)
         used, in_used = C.c_uint64(), C.c_uint64()
-        for attempt in range(2):
-            rc = lib.gb_bgzf_decompress_device(self._h, C.c_void_p(data.data_ptr()) if data.numel() else None, data.numel(),
-                                               1 if final else 0, C.c_void_p(out.data_ptr()), out.numel(), C.byref(used),
-                                               C.byref(in_used))
-            if rc != GB_ERR_CAPACITY or attempt:
-                break
-            out = torch.empty(max(1, used.value), dtype=torch.uint8, device=data.device)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_bgzf_decompress_device")
+        rc, out = _retry_on_capacity(
+            lambda o: lib.gb_bgzf_decompress_device(self._h, C.c_void_p(data.data_ptr()) if data.numel() else None, data.numel(),
+                                                    1 if final else 0, C.c_void_p(o.data_ptr()), o.numel(), C.byref(used), C.byref(in_used)),
+            out, lambda: torch.empty(max(1, used.value), dtype=torch.uint8, device=data.device))
+        _check(rc, "gb_bgzf_decompress_device")
         return out[: used.value], in_used.value
 
     def fastq_parse_device(self, texts, interleaved=False, final=True, max_reads=None, bases_cap=None, names_cap=None, quals=True):
@@ -999,15 +879,11 @@ class Device:
         used = (C.c_uint64 * len(texts))()
         n, mx = C.c_uint32(), C.c_uint32()
         torch.cuda.current_stream(dev).synchronize()
-        rc = lib.gb_fastq_parse_device(self._h, len(texts), ptrs, sizes, GB_FASTQ_INTERLEAVED if interleaved else 0, 1 if final else 0,
-                                       max_reads, C.c_void_p(reads.data_ptr()), C.c_void_p(q.data_ptr()) if quals else None, bases_cap,
-                                       C.c_void_p(read_off.data_ptr()), C.c_void_p(names.data_ptr()), names_cap,
-                                       C.c_void_p(name_off.data_ptr()), C.byref(n), C.byref(mx), used)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_fastq_parse_device")
-        rc = lib.gb_device_synchronize(self._h)
-        if rc != GB_OK:
-            raise GbError(rc, "gb_device_synchronize")
+        _check(lib.gb_fastq_parse_device(self._h, len(texts), ptrs, sizes, GB_FASTQ_INTERLEAVED if interleaved else 0, 1 if final else 0,
+                                         max_reads, C.c_void_p(reads.data_ptr()), C.c_void_p(q.data_ptr()) if quals else None, bases_cap,
+                                         C.c_void_p(read_off.data_ptr()), C.c_void_p(names.data_ptr()), names_cap,
+                                         C.c_void_p(name_off.data_ptr()), C.byref(n), C.byref(mx), used), "gb_fastq_parse_device")
+        _check(lib.gb_device_synchronize(self._h), "gb_device_synchronize")
         k = n.value
         nb, nn = int(read_off[k]), int(name_off[k])
         return {"reads": reads[:nb], "quals": q[:nb] if quals else None, "read_off": read_off[: k + 1], "names": names[:nn],

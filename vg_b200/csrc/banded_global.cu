@@ -69,37 +69,39 @@ extern "C" int gb_banded_global_batch(gb_device* d, uint32_t n,
                                       const uint8_t* query, const uint64_t* query_off, const int32_t* band_padding, const uint8_t* permissive,
                                       uint32_t map_cap, uint32_t edit_cap,
                                       int32_t* score, gb_mapping* maps, uint32_t* edits, uint32_t* n_maps, uint32_t* n_edits, uint8_t* status) {
-    if (!d || !node || !node_off || !pred || !pred_off || !query || !query_off || !band_padding || !permissive || !score || !maps ||
-        !edits || !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
-    if (n == 0) return GB_OK;
-    GB_CUDA(cudaSetDevice(d->device));
-    DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
-    int rc;
-    if ((rc = dag.validate(d, "gb_banded_global_batch"))) return rc;
-    std::vector<int32_t> pad(n);
-    for (uint32_t p = 0; p < n; p++) {
-        if (band_padding[p] < 0) { g_last_error = "gb_banded_global_batch: negative band padding"; return GB_ERR_ARG; }
-        // bands are int32 on the device: keep every diagonal within 2 * (m + bases) + 1
-        if (dag.bases[p] > (1u << 28)) { g_last_error = "gb_banded_global_batch: more than 2^28 bases in a problem"; return GB_ERR_ARG; }
-        // a padding of m + bases + 1 already puts every cell in the band, permissive or not, and masks no node;
-        // a wider one gives the same alignment
-        pad[p] = (int32_t)std::min<int64_t>(band_padding[p], (int64_t)dag.m[p] + (int64_t)dag.bases[p] + 1);
-    }
-    BgBatch b;
-    if ((rc = dag.check_limits("gb_banded_global_batch")) || (rc = dag.upload(d->stream, b.dag))) return rc;
-    SeamOutBufs out;
-    DevBuf<int32_t> d_pad, d_lastM, d_lastI, d_lastD; DevBuf<int64_t> d_sts, d_lts;
-    DevBuf<uint8_t> d_perm, d_argd, d_argh; DevBuf<BgNode> d_nd;
-    const uint64_t cols = dag.col_off[n] + 1, nodes = dag.total_nodes + 1;
-    if ((rc = d_pad.upload(pad.data(), n, d->stream)) || (rc = d_perm.upload(permissive, n, d->stream))) return rc;
-    if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
-    if ((rc = d_lastM.reserve(cols)) || (rc = d_lastI.reserve(cols)) || (rc = d_lastD.reserve(cols))) return rc;
-    if ((rc = d_argd.reserve(cols)) || (rc = d_argh.reserve(cols))) return rc;
-    if ((rc = d_nd.reserve(nodes)) || (rc = d_sts.reserve(nodes)) || (rc = d_lts.reserve(nodes))) return rc;
-    b.out = out.view;
-    b.pad = d_pad.ptr; b.permissive = d_perm.ptr;
-    b.nd = d_nd.ptr; b.sts = d_sts.ptr; b.lts = d_lts.ptr;
-    b.lastM = d_lastM.ptr; b.lastI = d_lastI.ptr; b.lastD = d_lastD.ptr; b.argd = d_argd.ptr; b.argh = d_argh.ptr;
-    if ((rc = launch_warp_per_problem(d, banded_global_kernel, b, BG_WARPS, bg_smem_per_warp(dag.Lc) * BG_WARPS))) return rc;
-    return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+    return gb::guarded("gb_banded_global_batch", [&] {
+        if (!d || !node || !node_off || !pred || !pred_off || !query || !query_off || !band_padding || !permissive || !score || !maps ||
+            !edits || !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
+        if (n == 0) return GB_OK;
+        GB_CUDA(cudaSetDevice(d->device));
+        DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
+        int rc;
+        if ((rc = dag.validate(d, "gb_banded_global_batch"))) return rc;
+        std::vector<int32_t> pad(n);
+        for (uint32_t p = 0; p < n; p++) {
+            if (band_padding[p] < 0) { g_last_error = "gb_banded_global_batch: negative band padding"; return GB_ERR_ARG; }
+            // bands are int32 on the device: keep every diagonal within 2 * (m + bases) + 1
+            if (dag.bases[p] > (1u << 28)) { g_last_error = "gb_banded_global_batch: more than 2^28 bases in a problem"; return GB_ERR_ARG; }
+            // a padding of m + bases + 1 already puts every cell in the band, permissive or not, and masks no node;
+            // a wider one gives the same alignment
+            pad[p] = (int32_t)std::min<int64_t>(band_padding[p], (int64_t)dag.m[p] + (int64_t)dag.bases[p] + 1);
+        }
+        BgBatch b;
+        if ((rc = dag.check_limits("gb_banded_global_batch")) || (rc = dag.upload(d->stream, b.dag))) return rc;
+        SeamOutBufs out;
+        DevBuf<int32_t> d_pad, d_lastM, d_lastI, d_lastD; DevBuf<int64_t> d_sts, d_lts;
+        DevBuf<uint8_t> d_perm, d_argd, d_argh; DevBuf<BgNode> d_nd;
+        const uint64_t cols = dag.col_off[n] + 1, nodes = dag.total_nodes + 1;
+        if ((rc = d_pad.upload(pad.data(), n, d->stream)) || (rc = d_perm.upload(permissive, n, d->stream))) return rc;
+        if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
+        if ((rc = d_lastM.reserve(cols)) || (rc = d_lastI.reserve(cols)) || (rc = d_lastD.reserve(cols))) return rc;
+        if ((rc = d_argd.reserve(cols)) || (rc = d_argh.reserve(cols))) return rc;
+        if ((rc = d_nd.reserve(nodes)) || (rc = d_sts.reserve(nodes)) || (rc = d_lts.reserve(nodes))) return rc;
+        b.out = out.view;
+        b.pad = d_pad.ptr; b.permissive = d_perm.ptr;
+        b.nd = d_nd.ptr; b.sts = d_sts.ptr; b.lts = d_lts.ptr;
+        b.lastM = d_lastM.ptr; b.lastI = d_lastI.ptr; b.lastD = d_lastD.ptr; b.argd = d_argd.ptr; b.argh = d_argh.ptr;
+        if ((rc = launch_warp_per_problem(d, banded_global_kernel, b, BG_WARPS, bg_smem_per_warp(dag.Lc) * BG_WARPS))) return rc;
+        return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+    });
 }

@@ -459,8 +459,6 @@ __global__ void bgzf_gather_kernel(const uint8_t* __restrict__ slots, const uint
     }
 }
 
-inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 int bgzf_compress_device(gb_device* d, const void* d_in, uint64_t in_bytes, void* d_out, uint64_t out_cap, uint64_t* out_used) {
     if (!d || !out_used || (!d_in && in_bytes) || !d_out) return GB_ERR_ARG;
     GB_CUDA(cudaSetDevice(d->device));
@@ -468,24 +466,24 @@ int bgzf_compress_device(gb_device* d, const void* d_in, uint64_t in_bytes, void
     const uint32_t grid = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(nb, 1), (uint64_t)d->n_sms);
     size_t scan = 0;
     GB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int64_t)(nb + 1), d->stream));
-    // workspace: total, member_bytes[nb + 1], off[nb + 1], scan temp, token slots (one block of u32 per CTA), member slots
-    const size_t o_sizes = 256, o_off = o_sizes + align256(8 * (nb + 1)), o_tmp = o_off + align256(8 * (nb + 1)),
-                 o_tok = o_tmp + align256(scan), o_slots = o_tok + align256((size_t)grid * BGZF_BLOCK * 4),
-                 ws_bytes = o_slots + (size_t)nb * BGZF_SLOT;
-    int rc;
-    if ((rc = d->bgzf_ws.reserve(ws_bytes))) return rc;
-    uint8_t* ws = d->bgzf_ws.ptr;
-    uint64_t* sizes = (uint64_t*)(ws + o_sizes);
-    uint64_t* off = (uint64_t*)(ws + o_off);
+    // workspace: total (not read: the host takes it from off[nb]), member_bytes[nb + 1], off[nb + 1], scan temp, token slots
+    // (one block of u32 per CTA), member slots
+    uint64_t *sizes, *off;
+    uint32_t* tok;
+    uint8_t *tmp, *slots;
+    int rc = carve(d->bgzf_ws, [&](Carve& c) {
+        c.take<uint64_t>(1); sizes = c.take<uint64_t>(nb + 1); off = c.take<uint64_t>(nb + 1); tmp = c.take<uint8_t>(scan);
+        tok = c.take<uint32_t>((size_t)grid * BGZF_BLOCK); slots = c.take<uint8_t>((size_t)nb * BGZF_SLOT);
+    });
+    if (rc) return rc;
     GB_CUDA(cudaFuncSetAttribute(bgzf_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SM_BYTES));
     GB_CUDA(cudaMemsetAsync(sizes + nb, 0, sizeof(uint64_t), d->stream));
     if (nb) {
-        bgzf_block_kernel<<<grid, BGZF_THREADS, SM_BYTES, d->stream>>>((const uint8_t*)d_in, in_bytes, nb, ws + o_slots,
-                                                                       (uint32_t*)(ws + o_tok), sizes);
+        bgzf_block_kernel<<<grid, BGZF_THREADS, SM_BYTES, d->stream>>>((const uint8_t*)d_in, in_bytes, nb, slots, tok, sizes);
         d->launches++;
         GB_CUDA(cudaGetLastError());
     }
-    GB_CUDA(cub::DeviceScan::ExclusiveSum(ws + o_tmp, scan, sizes, off, (int64_t)(nb + 1), d->stream));
+    GB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan, sizes, off, (int64_t)(nb + 1), d->stream));
     d->launches++;
     uint64_t h_total = 0;
     GB_CUDA(cudaMemcpyAsync(&h_total, off + nb, sizeof h_total, cudaMemcpyDeviceToHost, d->stream));
@@ -494,7 +492,7 @@ int bgzf_compress_device(gb_device* d, const void* d_in, uint64_t in_bytes, void
     *out_used = total;
     if (total > out_cap) { g_last_error = "gb_bgzf_compress_device: output capacity too small (*out_used holds the bytes needed)"; return GB_ERR_CAPACITY; }
     const uint32_t ggrid = (uint32_t)std::min<uint64_t>(nb + 1, (uint64_t)d->n_sms * 16);
-    bgzf_gather_kernel<<<ggrid, 256, 0, d->stream>>>(ws + o_slots, sizes, off, nb, (uint8_t*)d_out);
+    bgzf_gather_kernel<<<ggrid, 256, 0, d->stream>>>(slots, sizes, off, nb, (uint8_t*)d_out);
     d->launches++;
     GB_CUDA(cudaGetLastError());
     return GB_OK;
@@ -504,6 +502,5 @@ int bgzf_compress_device(gb_device* d, const void* d_in, uint64_t in_bytes, void
 } // namespace gb
 
 extern "C" int gb_bgzf_compress_device(gb_device* dev, const void* d_in, uint64_t in_bytes, void* d_out, uint64_t out_cap, uint64_t* out_used) {
-    try { return gb::bgzf_compress_device(dev, d_in, in_bytes, d_out, out_cap, out_used); }
-    catch (...) { return GB_ERR_CAPACITY; }
+    return gb::guarded("gb_bgzf_compress_device", [&] { return gb::bgzf_compress_device(dev, d_in, in_bytes, d_out, out_cap, out_used); });
 }

@@ -333,19 +333,15 @@ bgzf_inflate_kernel(const uint8_t* __restrict__ in, const Member* __restrict__ m
     }
 }
 
-inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 int bgzf_decompress_device(gb_device* d, const void* d_in, uint64_t in_bytes, int final, void* d_out, uint64_t out_cap,
                            uint64_t* out_used, uint64_t* in_used) {
     if (!d || !out_used || !in_used || (!d_in && in_bytes) || (!d_out && out_cap)) return GB_ERR_ARG;
     *out_used = 0; *in_used = 0;
     GB_CUDA(cudaSetDevice(d->device));
     const uint64_t cap = in_bytes / MIN_MEMBER + 1;
-    const size_t o_mem = 256, ws_bytes = o_mem + align256(sizeof(Member) * cap);
-    int rc;
-    if ((rc = d->inflate_ws.reserve(ws_bytes))) return rc;
-    WalkSum* sum = (WalkSum*)d->inflate_ws.ptr;
-    Member* mem = (Member*)(d->inflate_ws.ptr + o_mem);
+    WalkSum* sum;
+    Member* mem;
+    if (int rc = carve(d->inflate_ws, [&](Carve& c) { sum = c.take<WalkSum>(1); mem = c.take<Member>(cap); })) return rc;
     bgzf_walk_kernel<<<1, 1, 0, d->stream>>>((const uint8_t*)d_in, in_bytes, cap, mem, sum);
     d->launches++;
     GB_CUDA(cudaGetLastError());
@@ -390,6 +386,6 @@ int bgzf_decompress_device(gb_device* d, const void* d_in, uint64_t in_bytes, in
 
 extern "C" int gb_bgzf_decompress_device(gb_device* dev, const void* d_in, uint64_t in_bytes, int final, void* d_out,
                                          uint64_t out_cap, uint64_t* out_used, uint64_t* in_used) {
-    try { return gb::bgzf_decompress_device(dev, d_in, in_bytes, final, d_out, out_cap, out_used, in_used); }
-    catch (...) { return GB_ERR_CAPACITY; }
+    return gb::guarded("gb_bgzf_decompress_device",
+                       [&] { return gb::bgzf_decompress_device(dev, d_in, in_bytes, final, d_out, out_cap, out_used, in_used); });
 }

@@ -15,10 +15,8 @@
 
 namespace gb {
 
-thread_local std::string g_last_error;
-
 int fail_cuda(cudaError_t e, const char* what) {
-    g_last_error = std::string(what) + ": " + cudaGetErrorString(e);
+    set_last_error(what, ": ", cudaGetErrorString(e));
     return (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver) ? GB_ERR_NO_DEVICE : GB_ERR_CUDA;
 }
 
@@ -148,93 +146,95 @@ using namespace gb;
 extern "C" const char* gb_last_error(void) { return g_last_error.c_str(); }
 
 extern "C" int gb_device_create(const gb_flat_index* ix, int device_ordinal, gb_device** out) {
-    if (!ix || !out) return GB_ERR_ARG;
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) {
-        g_last_error = "no CUDA device available (libgiraffe_b200 has no CPU fallback)";
-        return GB_ERR_NO_DEVICE;
-    }
-    if (device_ordinal < 0 || device_ordinal >= ndev) return GB_ERR_ARG;
-    if ((ix->table_cells & (ix->table_cells - 1)) != 0) return GB_ERR_FORMAT;
-    GB_CUDA(cudaSetDevice(device_ordinal));
-    auto* d = new gb_device();
-    d->device = device_ordinal;
-    cudaDeviceProp prop;
-    GB_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
-    d->n_sms = prop.multiProcessorCount;
-    if (const char* env = std::getenv("GIRAFFE_B200_MAP_CHUNK")) {
-        const unsigned long v = std::strtoul(env, nullptr, 10);
-        if (v >= 2 && v <= (1ul << 24)) d->map_chunk = (uint32_t)(v & ~1ul);
-    }
-    if (const char* env = std::getenv("GIRAFFE_B200_TILES")) d->use_tiles = std::atoi(env) != 0;
-    if (const char* env = std::getenv("GIRAFFE_B200_POOL_SCALE")) {
-        const double v = std::strtod(env, nullptr);
-        if (v > 0.0 && v <= 1024.0) d->pool_scale = v;
-    }
-    if (const char* env = std::getenv("GIRAFFE_B200_SEED_TABLES")) {
-        unsigned mc = 0, cc = 0, ns = 64;
-        if (std::sscanf(env, "%u,%u,%u", &mc, &cc, &ns) >= 2 && mc >= 2 && cc >= 1) {
-            d->seed_mc = std::max<uint32_t>(16u, std::min<uint32_t>(gb::MAX_MINIMIZERS, (mc + 7u) & ~7u));
-            d->seed_cc = std::min<uint32_t>(64u, cc);
-            d->seed_ns = std::min<uint32_t>(64u, ns);
+    return gb::guarded("gb_device_create", [&] {
+        if (!ix || !out) return GB_ERR_ARG;
+        int ndev = 0;
+        cudaError_t e = cudaGetDeviceCount(&ndev);
+        if (e != cudaSuccess || ndev == 0) {
+            g_last_error = "no CUDA device available (libgiraffe_b200 has no CPU fallback)";
+            return GB_ERR_NO_DEVICE;
         }
-    }
-    GB_CUDA(cudaStreamCreateWithFlags(&d->own_stream, cudaStreamNonBlocking));
-    d->stream = d->own_stream;
-    for (int i = 0; i < 5; i++) GB_CUDA(cudaEventCreate(&d->ev_stage[i]));
-    GB_CUDA(cudaEventCreate(&d->ev0)); GB_CUDA(cudaEventCreate(&d->ev1));
-    GB_CUDA(cudaStreamCreateWithFlags(&d->s_in, cudaStreamNonBlocking));
-    GB_CUDA(cudaStreamCreateWithFlags(&d->s_out, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-        GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_in, cudaEventDisableTiming));
-        GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_done, cudaEventDisableTiming));
-        GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_hdr, cudaEventDisableTiming));
-        GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_out, cudaEventDisableTiming));
-        GB_CUDA(cudaEventCreate(&d->io[i].ev_k0)); GB_CUDA(cudaEventCreate(&d->io[i].ev_k1));
-    }
-    GB_CUDA(cudaMallocHost(&d->h_totals, 6 * sizeof(uint64_t)));
-    int rc;
-    if ((rc = d->nodes.upload(ix->nodes, ix->n_nodes, d->stream))) return rc;
-    if ((rc = d->seq.upload(ix->seq, ix->seq_bytes, d->stream))) return rc;
-    if ((rc = d->gbwt.upload(ix->gbwt, ix->gbwt_words, d->stream))) return rc;
-    if ((rc = d->dist.upload(ix->dist, ix->n_nodes / 2, d->stream))) return rc;
-    if ((rc = d->table.upload(ix->table, ix->table_cells, d->stream))) return rc;
-    if ((rc = d->hits.upload(ix->hits, ix->n_hits ? ix->n_hits : 1, d->stream, ix->n_hits))) return rc;
-    GB_CUDA(cudaStreamSynchronize(d->stream));
-    {
-        // ids in chain order (the rescue subgraph is cut from it, minimizer_mapper.cpp:3364)
-        std::vector<uint32_t> order;
-        for (uint32_t id = 1; id < ix->n_nodes / 2; id++) if (ix->nodes[2 * id].len > 0) order.push_back(id);
-        std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
-            const gb_dist_payload& pa = ix->dist[a]; const gb_dist_payload& pb = ix->dist[b];
-            if (pa.component != pb.component) return pa.component < pb.component;
-            if (pa.slot != pb.slot) return pa.slot < pb.slot;
-            if (pa.allele != pb.allele) return pa.allele < pb.allele;      // place inside the site = topological
-            return a < b;
-        });
-        if ((rc = d->slot_order.upload(order.data(), order.size() ? order.size() : 1, d->stream, order.size()))) return rc;
+        if (device_ordinal < 0 || device_ordinal >= ndev) return GB_ERR_ARG;
+        if ((ix->table_cells & (ix->table_cells - 1)) != 0) return GB_ERR_FORMAT;
+        GB_CUDA(cudaSetDevice(device_ordinal));
+        auto* d = new gb_device();
+        d->device = device_ordinal;
+        cudaDeviceProp prop;
+        GB_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
+        d->n_sms = prop.multiProcessorCount;
+        if (const char* env = std::getenv("GIRAFFE_B200_MAP_CHUNK")) {
+            const unsigned long v = std::strtoul(env, nullptr, 10);
+            if (v >= 2 && v <= (1ul << 24)) d->map_chunk = (uint32_t)(v & ~1ul);
+        }
+        if (const char* env = std::getenv("GIRAFFE_B200_TILES")) d->use_tiles = std::atoi(env) != 0;
+        if (const char* env = std::getenv("GIRAFFE_B200_POOL_SCALE")) {
+            const double v = std::strtod(env, nullptr);
+            if (v > 0.0 && v <= 1024.0) d->pool_scale = v;
+        }
+        if (const char* env = std::getenv("GIRAFFE_B200_SEED_TABLES")) {
+            unsigned mc = 0, cc = 0, ns = 64;
+            if (std::sscanf(env, "%u,%u,%u", &mc, &cc, &ns) >= 2 && mc >= 2 && cc >= 1) {
+                d->seed_mc = std::max<uint32_t>(16u, std::min<uint32_t>(gb::MAX_MINIMIZERS, (mc + 7u) & ~7u));
+                d->seed_cc = std::min<uint32_t>(64u, cc);
+                d->seed_ns = std::min<uint32_t>(64u, ns);
+            }
+        }
+        GB_CUDA(cudaStreamCreateWithFlags(&d->own_stream, cudaStreamNonBlocking));
+        d->stream = d->own_stream;
+        for (int i = 0; i < 5; i++) GB_CUDA(cudaEventCreate(&d->ev_stage[i]));
+        GB_CUDA(cudaEventCreate(&d->ev0)); GB_CUDA(cudaEventCreate(&d->ev1));
+        GB_CUDA(cudaStreamCreateWithFlags(&d->s_in, cudaStreamNonBlocking));
+        GB_CUDA(cudaStreamCreateWithFlags(&d->s_out, cudaStreamNonBlocking));
+        for (int i = 0; i < 2; i++) {
+            GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_in, cudaEventDisableTiming));
+            GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_done, cudaEventDisableTiming));
+            GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_hdr, cudaEventDisableTiming));
+            GB_CUDA(cudaEventCreateWithFlags(&d->io[i].ev_out, cudaEventDisableTiming));
+            GB_CUDA(cudaEventCreate(&d->io[i].ev_k0)); GB_CUDA(cudaEventCreate(&d->io[i].ev_k1));
+        }
+        GB_CUDA(cudaMallocHost(&d->h_totals, 6 * sizeof(uint64_t)));
+        int rc;
+        if ((rc = d->nodes.upload(ix->nodes, ix->n_nodes, d->stream))) return rc;
+        if ((rc = d->seq.upload(ix->seq, ix->seq_bytes, d->stream))) return rc;
+        if ((rc = d->gbwt.upload(ix->gbwt, ix->gbwt_words, d->stream))) return rc;
+        if ((rc = d->dist.upload(ix->dist, ix->n_nodes / 2, d->stream))) return rc;
+        if ((rc = d->table.upload(ix->table, ix->table_cells, d->stream))) return rc;
+        if ((rc = d->hits.upload(ix->hits, ix->n_hits ? ix->n_hits : 1, d->stream, ix->n_hits))) return rc;
         GB_CUDA(cudaStreamSynchronize(d->stream));
-        d->ix.slot_order = d->slot_order.ptr; d->ix.n_ids = (uint32_t)order.size();
-    }
-    if (ix->n_slots) {
-        if ((rc = d->slots.upload(ix->slots, ix->n_slots, d->stream))) return rc;
-        if ((rc = d->site_dist.upload(ix->site_dist, ix->site_dist_len ? ix->site_dist_len : 1, d->stream, ix->site_dist_len))) return rc;
-        GB_CUDA(cudaStreamSynchronize(d->stream));
-        d->h_slots.assign(ix->slots, ix->slots + ix->n_slots);
-        d->h_site_dist.assign(ix->site_dist, ix->site_dist + ix->site_dist_len);
-    }
-    d->ix.slots = ix->n_slots ? d->slots.ptr : nullptr; d->ix.n_slots = (uint32_t)ix->n_slots; d->ix.site_dist = ix->n_slots ? d->site_dist.ptr : nullptr;
-    d->h_node_len.resize(ix->n_nodes);
-    d->h_dist.assign(ix->dist, ix->dist + ix->n_nodes / 2);
-    for (uint32_t v = 0; v < ix->n_nodes; v++) d->h_node_len[v] = ix->nodes[v].len;
-    d->ix.nodes = d->nodes.ptr; d->ix.seq = d->seq.ptr; d->ix.gbwt = d->gbwt.ptr; d->ix.dist = d->dist.ptr;
-    d->ix.table = d->table.ptr; d->ix.hits = d->hits.ptr;
-    d->ix.table_mask = ix->table_cells - 1; d->ix.n_nodes = ix->n_nodes; d->ix.k = ix->k; d->ix.w = ix->w;
-    d->sc = DevScores{1, 4, 6, 1, 5};
-    GB_CUDA(cudaMalloc(&d->work_counter, 64));
-    *out = d;
-    return GB_OK;
+        {
+            // ids in chain order (the rescue subgraph is cut from it, minimizer_mapper.cpp:3364)
+            std::vector<uint32_t> order;
+            for (uint32_t id = 1; id < ix->n_nodes / 2; id++) if (ix->nodes[2 * id].len > 0) order.push_back(id);
+            std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+                const gb_dist_payload& pa = ix->dist[a]; const gb_dist_payload& pb = ix->dist[b];
+                if (pa.component != pb.component) return pa.component < pb.component;
+                if (pa.slot != pb.slot) return pa.slot < pb.slot;
+                if (pa.allele != pb.allele) return pa.allele < pb.allele;      // place inside the site = topological
+                return a < b;
+            });
+            if ((rc = d->slot_order.upload(order.data(), order.size() ? order.size() : 1, d->stream, order.size()))) return rc;
+            GB_CUDA(cudaStreamSynchronize(d->stream));
+            d->ix.slot_order = d->slot_order.ptr; d->ix.n_ids = (uint32_t)order.size();
+        }
+        if (ix->n_slots) {
+            if ((rc = d->slots.upload(ix->slots, ix->n_slots, d->stream))) return rc;
+            if ((rc = d->site_dist.upload(ix->site_dist, ix->site_dist_len ? ix->site_dist_len : 1, d->stream, ix->site_dist_len))) return rc;
+            GB_CUDA(cudaStreamSynchronize(d->stream));
+            d->h_slots.assign(ix->slots, ix->slots + ix->n_slots);
+            d->h_site_dist.assign(ix->site_dist, ix->site_dist + ix->site_dist_len);
+        }
+        d->ix.slots = ix->n_slots ? d->slots.ptr : nullptr; d->ix.n_slots = (uint32_t)ix->n_slots; d->ix.site_dist = ix->n_slots ? d->site_dist.ptr : nullptr;
+        d->h_node_len.resize(ix->n_nodes);
+        d->h_dist.assign(ix->dist, ix->dist + ix->n_nodes / 2);
+        for (uint32_t v = 0; v < ix->n_nodes; v++) d->h_node_len[v] = ix->nodes[v].len;
+        d->ix.nodes = d->nodes.ptr; d->ix.seq = d->seq.ptr; d->ix.gbwt = d->gbwt.ptr; d->ix.dist = d->dist.ptr;
+        d->ix.table = d->table.ptr; d->ix.hits = d->hits.ptr;
+        d->ix.table_mask = ix->table_cells - 1; d->ix.n_nodes = ix->n_nodes; d->ix.k = ix->k; d->ix.w = ix->w;
+        d->sc = DevScores{1, 4, 6, 1, 5};
+        GB_CUDA(cudaMalloc(&d->work_counter, 64));
+        *out = d;
+        return GB_OK;
+    });
 }
 
 extern "C" void gb_device_destroy(gb_device* d) {
@@ -337,57 +337,59 @@ extern "C" int gb_extend_batch(gb_device* d, const gb_extend_params* hp,
                                const gb_seed* seeds, const uint64_t* seed_off,
                                uint32_t* ext_count, uint8_t* status,
                                gb_extension* ext, uint32_t* path_pool, uint32_t* mism_pool) {
-    if (!d || !hp || !reads || !read_off || !item_read || !seeds || !seed_off || !ext_count || !status || !ext ||
-        !path_pool || !mism_pool) return GB_ERR_ARG;
-    if (hp->max_ext_per_item == 0 || hp->path_cap_per_item == 0 || hp->mism_cap_per_item == 0) return GB_ERR_ARG;
-    if (n_items == 0) return GB_OK;
-    GB_CUDA(cudaSetDevice(d->device));
-    uint32_t max_len = 0;
-    for (uint32_t r = 0; r < n_reads; r++) max_len = std::max<uint32_t>(max_len, (uint32_t)(read_off[r + 1] - read_off[r]));
-    for (uint32_t i = 0; i < n_items; i++) if (item_read[i] >= n_reads) return GB_ERR_ARG;
-    const uint64_t n_seeds = seed_off[n_items];
+    return gb::guarded("gb_extend_batch", [&] {
+        if (!d || !hp || !reads || !read_off || !item_read || !seeds || !seed_off || !ext_count || !status || !ext ||
+            !path_pool || !mism_pool) return GB_ERR_ARG;
+        if (hp->max_ext_per_item == 0 || hp->path_cap_per_item == 0 || hp->mism_cap_per_item == 0) return GB_ERR_ARG;
+        if (n_items == 0) return GB_OK;
+        GB_CUDA(cudaSetDevice(d->device));
+        uint32_t max_len = 0;
+        for (uint32_t r = 0; r < n_reads; r++) max_len = std::max<uint32_t>(max_len, (uint32_t)(read_off[r + 1] - read_off[r]));
+        for (uint32_t i = 0; i < n_items; i++) if (item_read[i] >= n_reads) return GB_ERR_ARG;
+        const uint64_t n_seeds = seed_off[n_items];
 
-    DevBuf<uint8_t> d_reads; DevBuf<uint64_t> d_read_off, d_seed_off; DevBuf<uint32_t> d_item_read; DevBuf<gb_seed> d_seeds;
-    DevBuf<uint32_t> d_cnt, d_path, d_mism; DevBuf<uint8_t> d_status; DevBuf<gb_extension> d_ext;
-    int rc;
-    if ((rc = d_reads.upload(reads, read_off[n_reads] ? read_off[n_reads] : 1, d->stream, read_off[n_reads]))) return rc;
-    if ((rc = d_read_off.upload(read_off, n_reads + 1, d->stream))) return rc;
-    if ((rc = d_item_read.upload(item_read, n_items, d->stream))) return rc;
-    if ((rc = d_seeds.upload(seeds, n_seeds ? n_seeds : 1, d->stream, n_seeds))) return rc;
-    if ((rc = d_seed_off.upload(seed_off, n_items + 1, d->stream))) return rc;
-    if ((rc = d_cnt.reserve(n_items))) return rc;
-    if ((rc = d_status.reserve(n_items))) return rc;
-    if ((rc = d_ext.reserve((size_t)n_items * hp->max_ext_per_item))) return rc;
-    if ((rc = d_path.reserve((size_t)n_items * hp->path_cap_per_item))) return rc;
-    if ((rc = d_mism.reserve((size_t)n_items * hp->mism_cap_per_item))) return rc;
+        DevBuf<uint8_t> d_reads; DevBuf<uint64_t> d_read_off, d_seed_off; DevBuf<uint32_t> d_item_read; DevBuf<gb_seed> d_seeds;
+        DevBuf<uint32_t> d_cnt, d_path, d_mism; DevBuf<uint8_t> d_status; DevBuf<gb_extension> d_ext;
+        int rc;
+        if ((rc = d_reads.upload(reads, read_off[n_reads] ? read_off[n_reads] : 1, d->stream, read_off[n_reads]))) return rc;
+        if ((rc = d_read_off.upload(read_off, n_reads + 1, d->stream))) return rc;
+        if ((rc = d_item_read.upload(item_read, n_items, d->stream))) return rc;
+        if ((rc = d_seeds.upload(seeds, n_seeds ? n_seeds : 1, d->stream, n_seeds))) return rc;
+        if ((rc = d_seed_off.upload(seed_off, n_items + 1, d->stream))) return rc;
+        if ((rc = d_cnt.reserve(n_items))) return rc;
+        if ((rc = d_status.reserve(n_items))) return rc;
+        if ((rc = d_ext.reserve((size_t)n_items * hp->max_ext_per_item))) return rc;
+        if ((rc = d_path.reserve((size_t)n_items * hp->path_cap_per_item))) return rc;
+        if ((rc = d_mism.reserve((size_t)n_items * hp->mism_cap_per_item))) return rc;
 
-    ExtendParams p;
-    p.sc = d->sc; p.max_mismatches = hp->max_mismatches; p.overlap_threshold = hp->overlap_threshold;
-    p.overlap_threshold_unused = 0.f; p.trim = hp->trim;
-    p.max_ext = hp->max_ext_per_item; p.path_cap = hp->path_cap_per_item; p.mism_cap = hp->mism_cap_per_item;
-    ExtendBatch b{};
-    b.reads = d_reads.ptr; b.read_off = d_read_off.ptr; b.item_read = d_item_read.ptr;
-    b.seeds = d_seeds.ptr; b.seed_off = d_seed_off.ptr; b.n_items = n_items;
-    b.ext_count = d_cnt.ptr; b.status = d_status.ptr; b.ext = d_ext.ptr; b.path_pool = d_path.ptr; b.mism_pool = d_mism.ptr;
+        ExtendParams p;
+        p.sc = d->sc; p.max_mismatches = hp->max_mismatches; p.overlap_threshold = hp->overlap_threshold;
+        p.overlap_threshold_unused = 0.f; p.trim = hp->trim;
+        p.max_ext = hp->max_ext_per_item; p.path_cap = hp->path_cap_per_item; p.mism_cap = hp->mism_cap_per_item;
+        ExtendBatch b{};
+        b.reads = d_reads.ptr; b.read_off = d_read_off.ptr; b.item_read = d_item_read.ptr;
+        b.seeds = d_seeds.ptr; b.seed_off = d_seed_off.ptr; b.n_items = n_items;
+        b.ext_count = d_cnt.ptr; b.status = d_status.ptr; b.ext = d_ext.ptr; b.path_pool = d_path.ptr; b.mism_pool = d_mism.ptr;
 
-    GB_CUDA(cudaEventRecord(d->ev0, d->stream));
-    if ((rc = launch_extend(d, p, b, max_len))) return rc;
-    GB_CUDA(cudaEventRecord(d->ev1, d->stream));
+        GB_CUDA(cudaEventRecord(d->ev0, d->stream));
+        if ((rc = launch_extend(d, p, b, max_len))) return rc;
+        GB_CUDA(cudaEventRecord(d->ev1, d->stream));
 
-    GB_CUDA(cudaMemcpyAsync(ext_count, d_cnt.ptr, sizeof(uint32_t) * n_items, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(status, d_status.ptr, n_items, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(ext, d_ext.ptr, sizeof(gb_extension) * (size_t)n_items * hp->max_ext_per_item, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(path_pool, d_path.ptr, sizeof(uint32_t) * (size_t)n_items * hp->path_cap_per_item, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(mism_pool, d_mism.ptr, sizeof(uint32_t) * (size_t)n_items * hp->mism_cap_per_item, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaStreamSynchronize(d->stream));
-    GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
-    // make pool offsets absolute
-    for (uint32_t i = 0; i < n_items; i++) {
-        for (uint32_t j = 0; j < ext_count[i]; j++) {
-            gb_extension& e = ext[(size_t)i * hp->max_ext_per_item + j];
-            e.path_off += i * hp->path_cap_per_item;
-            e.mism_off += i * hp->mism_cap_per_item;
+        GB_CUDA(cudaMemcpyAsync(ext_count, d_cnt.ptr, sizeof(uint32_t) * n_items, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(status, d_status.ptr, n_items, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(ext, d_ext.ptr, sizeof(gb_extension) * (size_t)n_items * hp->max_ext_per_item, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(path_pool, d_path.ptr, sizeof(uint32_t) * (size_t)n_items * hp->path_cap_per_item, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(mism_pool, d_mism.ptr, sizeof(uint32_t) * (size_t)n_items * hp->mism_cap_per_item, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaStreamSynchronize(d->stream));
+        GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
+        // make pool offsets absolute
+        for (uint32_t i = 0; i < n_items; i++) {
+            for (uint32_t j = 0; j < ext_count[i]; j++) {
+                gb_extension& e = ext[(size_t)i * hp->max_ext_per_item + j];
+                e.path_off += i * hp->path_cap_per_item;
+                e.mism_off += i * hp->mism_cap_per_item;
+            }
         }
-    }
-    return GB_OK;
+        return GB_OK;
+    });
 }

@@ -380,11 +380,10 @@ extern "C" int gb_chain_batch(gb_device* d, const gb_chain_params* P, uint32_t n
                               const gb_chain_candidate* cands, const uint64_t* cand_off,
                               int32_t* dp_score, uint32_t* dp_source, uint64_t* dp_paths, uint32_t* dp_rec,
                               uint32_t* n_chains, int32_t* chain_score, uint32_t* chain_begin, uint32_t* chain_count, uint32_t* chain_items) {
-    try {
+    return gb::guarded("gb_chain_batch", [&] {
         return chain_batch_impl(d, P, n_problems, anchors, anchor_off, cands, cand_off, dp_score, dp_source, dp_paths, dp_rec,
                                 n_chains, chain_score, chain_begin, chain_count, chain_items, nullptr);
-    } catch (const std::bad_alloc&) { return GB_ERR_CAPACITY; }
-    catch (...) { return GB_ERR_ARG; }
+    });
 }
 
 extern "C" int gb_chain_batch_transitions(gb_device* d, const gb_chain_params* P, uint32_t n_problems,
@@ -393,105 +392,101 @@ extern "C" int gb_chain_batch_transitions(gb_device* d, const gb_chain_params* P
                                           int32_t* dp_score, uint32_t* dp_source, uint64_t* dp_paths, uint32_t* dp_rec,
                                           uint32_t* n_chains, int32_t* chain_score, uint32_t* chain_begin, uint32_t* chain_count, uint32_t* chain_items,
                                           uint32_t* candidate_indel) {
-    try {
+    return gb::guarded("gb_chain_batch_transitions", [&] {
         return chain_batch_impl(d, P, n_problems, anchors, anchor_off, cands, cand_off, dp_score, dp_source, dp_paths, dp_rec,
                                 n_chains, chain_score, chain_begin, chain_count, chain_items, candidate_indel);
-    } catch (const std::bad_alloc&) { return GB_ERR_CAPACITY; }
-    catch (...) { return GB_ERR_ARG; }
+    });
 }
 
 // MinimizerMapper::to_anchor, minimizer_mapper_from_chains.cpp:3978-4038 (host side: a few integer operations per seed)
 extern "C" int gb_chain_anchors(const gb_flat_index* ix, const gb_scores* scores, uint32_t n, const uint32_t* seed_pos,
                                 const uint32_t* min_offset, const uint8_t* min_is_reverse, const uint32_t* min_length,
                                 const uint64_t* paths, gb_chain_anchor* out) {
-    if (!ix || !scores || (n && (!seed_pos || !min_offset || !min_is_reverse || !min_length || !out))) return GB_ERR_ARG;
-    for (uint32_t i = 0; i < n; i++) {
-        const uint32_t v = seed_pos[2 * i], off = seed_pos[2 * i + 1], mlen = min_length[i];
-        if (v < 2 || v >= ix->n_nodes || ix->nodes[v].len == 0 || off >= ix->nodes[v].len || mlen == 0) { g_last_error = "gb_chain_anchors: seed outside the graph or empty minimizer"; return GB_ERR_ARG; }
-        uint32_t length, margin_left, margin_right, read_start, hint_start;
-        if (min_is_reverse[i]) {
-            const uint32_t end = off + 1;                              // the seed is the final base of the match: past-end position
-            length = std::min(mlen, end);                              // how much of the node lies before it
-            margin_left = mlen - length; margin_right = 0;
-            if (min_offset[i] + 1 < length) { g_last_error = "gb_chain_anchors: reverse minimizer runs off the read start"; return GB_ERR_ARG; }
-            read_start = min_offset[i] + 1 - length;
-            hint_start = length - 1;                                   // the seed is the last 1 bp interval
-        } else {
-            length = std::min(mlen, ix->nodes[v].len - off);           // how much of the node lies behind the seed
-            margin_left = 0; margin_right = mlen - length;
-            read_start = min_offset[i];
-            hint_start = 0;
+    return gb::guarded("gb_chain_anchors", [&] {
+        if (!ix || !scores || (n && (!seed_pos || !min_offset || !min_is_reverse || !min_length || !out))) return GB_ERR_ARG;
+        for (uint32_t i = 0; i < n; i++) {
+            const uint32_t v = seed_pos[2 * i], off = seed_pos[2 * i + 1], mlen = min_length[i];
+            if (v < 2 || v >= ix->n_nodes || ix->nodes[v].len == 0 || off >= ix->nodes[v].len || mlen == 0) { g_last_error = "gb_chain_anchors: seed outside the graph or empty minimizer"; return GB_ERR_ARG; }
+            uint32_t length, margin_left, margin_right, read_start, hint_start;
+            if (min_is_reverse[i]) {
+                const uint32_t end = off + 1;                              // the seed is the final base of the match: past-end position
+                length = std::min(mlen, end);                              // how much of the node lies before it
+                margin_left = mlen - length; margin_right = 0;
+                if (min_offset[i] + 1 < length) { g_last_error = "gb_chain_anchors: reverse minimizer runs off the read start"; return GB_ERR_ARG; }
+                read_start = min_offset[i] + 1 - length;
+                hint_start = length - 1;                                   // the seed is the last 1 bp interval
+            } else {
+                length = std::min(mlen, ix->nodes[v].len - off);           // how much of the node lies behind the seed
+                margin_left = 0; margin_right = mlen - length;
+                read_start = min_offset[i];
+                hint_start = 0;
+            }
+            gb_chain_anchor a;
+            a.read_start = read_start; a.length = length; a.margin_before = margin_left; a.margin_after = margin_right;
+            a.score = (int32_t)scores->match * (int32_t)(margin_left + length + margin_right);        // score_exact_match over the whole minimizer
+            a.start_hint_offset = hint_start; a.end_hint_offset = length - hint_start; a.base_seed_length = margin_left + length + margin_right;
+            a.start_paths = a.end_paths = paths ? paths[i] : 0;
+            out[i] = a;
         }
-        gb_chain_anchor a;
-        a.read_start = read_start; a.length = length; a.margin_before = margin_left; a.margin_after = margin_right;
-        a.score = (int32_t)scores->match * (int32_t)(margin_left + length + margin_right);        // score_exact_match over the whole minimizer
-        a.start_hint_offset = hint_start; a.end_hint_offset = length - hint_start; a.base_seed_length = margin_left + length + margin_right;
-        a.start_paths = a.end_paths = paths ? paths[i] : 0;
-        out[i] = a;
-    }
-    return GB_OK;
-}
-
-static int chain_candidates_impl(gb_device* d, uint32_t n_problems, const uint32_t* seed_pos, const uint64_t* seed_off,
-                                 uint64_t limit, gb_chain_candidate* candidates, uint64_t candidate_cap, uint64_t* cand_off) {
-    if (!d || !seed_off || !cand_off || (candidate_cap && !candidates)) return GB_ERR_ARG;
-    for (uint32_t p = 0; p <= n_problems; p++) cand_off[p] = 0;
-    if (n_problems == 0) return GB_OK;
-    const uint64_t total = seed_off[n_problems];
-    if (total >= 0x7ffffff0ull || (total && !seed_pos)) return GB_ERR_ARG;
-    if (total == 0) return GB_OK;
-    std::vector<uint32_t> pb(total), pe(total);
-    for (uint32_t p = 0; p < n_problems; p++) {
-        if (seed_off[p + 1] < seed_off[p]) return GB_ERR_ARG;
-        if (seed_off[p + 1] - seed_off[p] > GB_CHAIN_MAX_ANCHORS) { g_last_error = "gb_chain_candidates_batch: more than GB_CHAIN_MAX_ANCHORS seeds in one problem"; return GB_ERR_ARG; }
-        for (uint64_t i = seed_off[p]; i < seed_off[p + 1]; i++) {
-            const uint32_t v = seed_pos[2 * i], o = seed_pos[2 * i + 1];
-            if (v < 2 || v >= d->h_node_len.size() || d->h_node_len[v] == 0 || o >= d->h_node_len[v]) { g_last_error = "gb_chain_candidates_batch: seed position outside the graph"; return GB_ERR_ARG; }
-            pb[i] = (uint32_t)seed_off[p]; pe[i] = (uint32_t)seed_off[p + 1];
-        }
-    }
-    GB_CUDA(cudaSetDevice(d->device));
-    DevBuf<uint32_t> d_pos, d_pb, d_pe; DevBuf<uint64_t> d_count, d_offset; DevBuf<uint8_t> d_tmp; DevBuf<gb_chain_candidate> d_out;
-    int rc;
-    if ((rc = d_pos.upload(seed_pos, 2 * total, d->stream)) || (rc = d_pb.upload(pb.data(), total, d->stream)) || (rc = d_pe.upload(pe.data(), total, d->stream)) ||
-        (rc = d_count.reserve(total + 1)) || (rc = d_offset.reserve(total + 1))) return rc;
-    GB_CUDA(cudaMemsetAsync(d_count.ptr + total, 0, sizeof(uint64_t), d->stream));
-    CandBatch b; b.n_seeds = (uint32_t)total; b.pos = d_pos.ptr; b.prob_begin = d_pb.ptr; b.prob_end = d_pe.ptr; b.limit = limit;
-    b.count = d_count.ptr; b.offset = d_offset.ptr; b.out = nullptr;
-    const uint32_t grid = std::max<uint32_t>(1u, std::min<uint32_t>((uint32_t)d->n_sms * 16, (uint32_t)((total + 3) / 4)));
-    GB_CUDA(cudaEventRecord(d->ev0, d->stream));
-    chain_candidates_kernel<false><<<grid, 128, 0, d->stream>>>(d->ix, b);
-    d->launches++;
-    GB_CUDA(cudaGetLastError());
-    size_t tmp_bytes = 0;
-    GB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_count.ptr, d_offset.ptr, (int)(total + 1), d->stream));
-    if ((rc = d_tmp.reserve(tmp_bytes + 256))) return rc;
-    size_t tb = d_tmp.cap;
-    GB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp.ptr, tb, d_count.ptr, d_offset.ptr, (int)(total + 1), d->stream));
-    d->launches++;
-    std::vector<uint64_t> h_off(total + 1);
-    GB_CUDA(cudaMemcpyAsync(h_off.data(), d_offset.ptr, sizeof(uint64_t) * (total + 1), cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaStreamSynchronize(d->stream));
-    for (uint32_t p = 0; p <= n_problems; p++) cand_off[p] = h_off[seed_off[p]];
-    const uint64_t n_out = h_off[total];
-    if (n_out > candidate_cap) { g_last_error = "gb_chain_candidates_batch: candidate capacity too small (cand_off holds the sizes needed)"; return GB_ERR_CAPACITY; }
-    if (n_out) {
-        if ((rc = d_out.reserve(n_out))) return rc;
-        b.out = d_out.ptr;
-        chain_candidates_kernel<true><<<grid, 128, 0, d->stream>>>(d->ix, b);
-        d->launches++;
-        GB_CUDA(cudaGetLastError());
-        GB_CUDA(cudaEventRecord(d->ev1, d->stream));
-        GB_CUDA(cudaMemcpyAsync(candidates, d_out.ptr, sizeof(gb_chain_candidate) * n_out, cudaMemcpyDeviceToHost, d->stream));
-    } else GB_CUDA(cudaEventRecord(d->ev1, d->stream));
-    GB_CUDA(cudaStreamSynchronize(d->stream));
-    GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
-    return GB_OK;
+        return GB_OK;
+    });
 }
 
 extern "C" int gb_chain_candidates_batch(gb_device* d, uint32_t n_problems, const uint32_t* seed_pos, const uint64_t* seed_off,
-                                         uint64_t max_graph_lookback_bases, gb_chain_candidate* candidates, uint64_t candidate_cap, uint64_t* cand_off) {
-    try { return chain_candidates_impl(d, n_problems, seed_pos, seed_off, max_graph_lookback_bases, candidates, candidate_cap, cand_off); }
-    catch (const std::bad_alloc&) { return GB_ERR_CAPACITY; }
-    catch (...) { return GB_ERR_ARG; }
+                                         uint64_t limit, gb_chain_candidate* candidates, uint64_t candidate_cap, uint64_t* cand_off) {
+    return gb::guarded("gb_chain_candidates_batch", [&] {
+        if (!d || !seed_off || !cand_off || (candidate_cap && !candidates)) return GB_ERR_ARG;
+        for (uint32_t p = 0; p <= n_problems; p++) cand_off[p] = 0;
+        if (n_problems == 0) return GB_OK;
+        const uint64_t total = seed_off[n_problems];
+        if (total >= 0x7ffffff0ull || (total && !seed_pos)) return GB_ERR_ARG;
+        if (total == 0) return GB_OK;
+        std::vector<uint32_t> pb(total), pe(total);
+        for (uint32_t p = 0; p < n_problems; p++) {
+            if (seed_off[p + 1] < seed_off[p]) return GB_ERR_ARG;
+            if (seed_off[p + 1] - seed_off[p] > GB_CHAIN_MAX_ANCHORS) { g_last_error = "gb_chain_candidates_batch: more than GB_CHAIN_MAX_ANCHORS seeds in one problem"; return GB_ERR_ARG; }
+            for (uint64_t i = seed_off[p]; i < seed_off[p + 1]; i++) {
+                const uint32_t v = seed_pos[2 * i], o = seed_pos[2 * i + 1];
+                if (v < 2 || v >= d->h_node_len.size() || d->h_node_len[v] == 0 || o >= d->h_node_len[v]) { g_last_error = "gb_chain_candidates_batch: seed position outside the graph"; return GB_ERR_ARG; }
+                pb[i] = (uint32_t)seed_off[p]; pe[i] = (uint32_t)seed_off[p + 1];
+            }
+        }
+        GB_CUDA(cudaSetDevice(d->device));
+        DevBuf<uint32_t> d_pos, d_pb, d_pe; DevBuf<uint64_t> d_count, d_offset; DevBuf<uint8_t> d_tmp; DevBuf<gb_chain_candidate> d_out;
+        int rc;
+        if ((rc = d_pos.upload(seed_pos, 2 * total, d->stream)) || (rc = d_pb.upload(pb.data(), total, d->stream)) || (rc = d_pe.upload(pe.data(), total, d->stream)) ||
+            (rc = d_count.reserve(total + 1)) || (rc = d_offset.reserve(total + 1))) return rc;
+        GB_CUDA(cudaMemsetAsync(d_count.ptr + total, 0, sizeof(uint64_t), d->stream));
+        CandBatch b; b.n_seeds = (uint32_t)total; b.pos = d_pos.ptr; b.prob_begin = d_pb.ptr; b.prob_end = d_pe.ptr; b.limit = limit;
+        b.count = d_count.ptr; b.offset = d_offset.ptr; b.out = nullptr;
+        const uint32_t grid = std::max<uint32_t>(1u, std::min<uint32_t>((uint32_t)d->n_sms * 16, (uint32_t)((total + 3) / 4)));
+        GB_CUDA(cudaEventRecord(d->ev0, d->stream));
+        chain_candidates_kernel<false><<<grid, 128, 0, d->stream>>>(d->ix, b);
+        d->launches++;
+        GB_CUDA(cudaGetLastError());
+        size_t tmp_bytes = 0;
+        GB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_count.ptr, d_offset.ptr, (int)(total + 1), d->stream));
+        if ((rc = d_tmp.reserve(tmp_bytes + 256))) return rc;
+        size_t tb = d_tmp.cap;
+        GB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp.ptr, tb, d_count.ptr, d_offset.ptr, (int)(total + 1), d->stream));
+        d->launches++;
+        std::vector<uint64_t> h_off(total + 1);
+        GB_CUDA(cudaMemcpyAsync(h_off.data(), d_offset.ptr, sizeof(uint64_t) * (total + 1), cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaStreamSynchronize(d->stream));
+        for (uint32_t p = 0; p <= n_problems; p++) cand_off[p] = h_off[seed_off[p]];
+        const uint64_t n_out = h_off[total];
+        if (n_out > candidate_cap) { g_last_error = "gb_chain_candidates_batch: candidate capacity too small (cand_off holds the sizes needed)"; return GB_ERR_CAPACITY; }
+        if (n_out) {
+            if ((rc = d_out.reserve(n_out))) return rc;
+            b.out = d_out.ptr;
+            chain_candidates_kernel<true><<<grid, 128, 0, d->stream>>>(d->ix, b);
+            d->launches++;
+            GB_CUDA(cudaGetLastError());
+            GB_CUDA(cudaEventRecord(d->ev1, d->stream));
+            GB_CUDA(cudaMemcpyAsync(candidates, d_out.ptr, sizeof(gb_chain_candidate) * n_out, cudaMemcpyDeviceToHost, d->stream));
+        } else GB_CUDA(cudaEventRecord(d->ev1, d->stream));
+        GB_CUDA(cudaStreamSynchronize(d->stream));
+        GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
+        return GB_OK;
+    });
 }

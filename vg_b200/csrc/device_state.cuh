@@ -1,6 +1,7 @@
 // device_state.cuh — the opaque gb_device handle: HBM-resident index, stream, workspaces.
 #pragma once
 #include "giraffe_b200.h"
+#include "entry_guard.h"
 #include "device_index.cuh"
 #include "extend.cuh"
 #include "map_state.cuh"
@@ -18,7 +19,6 @@ constexpr int EXTEND_WARPS = 8;           // warps per CTA of the extension kern
 constexpr uint32_t EXTEND_Q_CAP = 512;    // frontier entries per warp (64 B each)
 constexpr uint32_t EXTEND_A_CAP = 4096;   // path-arena nodes per warp (8 B each)
 
-extern thread_local std::string g_last_error;
 int fail_cuda(cudaError_t e, const char* what);
 
 #define GB_CUDA(call)                                                        \
@@ -58,6 +58,29 @@ struct DevBuf {
         return GB_OK;
     }
 };
+
+// Typed slices of one workspace, each starting on a 256-byte boundary (CUB's temp storage is one more slice).  Without a
+// base it only adds up the bytes, so carve() below runs the same layout once to size the buffer and once to bind it.
+struct Carve {
+    uint8_t* base;
+    size_t bytes = 0;
+    template <typename T> T* take(size_t n) {
+        T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+        bytes += (n * sizeof(T) + 255) & ~(size_t)255;
+        return p;
+    }
+};
+
+// Reserves `ws` for the slices `layout(Carve&)` takes, then binds them to it (the pattern of cub::AliasTemporaries).
+template <typename Layout>
+int carve(DevBuf<uint8_t>& ws, Layout&& layout) {
+    Carve size{nullptr};
+    layout(size);
+    if (int rc = ws.reserve(size.bytes)) return rc;
+    Carve bind{ws.ptr};
+    layout(bind);
+    return GB_OK;
+}
 
 // The mapping pipeline's device counters, zeroed at the start of every map_device call: work counters that hand units
 // to the persistent kernels, and the cursors and counts of what the kernels appended to the pools and lists.  The

@@ -10,6 +10,7 @@
 // giraffe_main.cpp:2209-2226 hands alignments to an AlignmentEmitter; this is the stand-in until the shim converts
 // records to vg::Alignment itself (INTEGRATION.md §2).  PARITY UNPINNED: no libvgio here to compare bytes with.
 #include "giraffe_b200.h"
+#include "entry_guard.h"
 
 #include <algorithm>
 #include <cstdio>
@@ -319,8 +320,8 @@ static int gb_emit_gam_impl(const gb_flat_index* ix, uint32_t n, const gb_alignm
     extern "C" int NAME(const gb_flat_index* ix, uint32_t n, const gb_alignment* aln, const gb_mapping* mappings, uint64_t mapping_pool_len, \
                         const uint32_t* edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* reads, const uint8_t* quals,         \
                         const uint64_t* read_off, const uint8_t* names, const uint64_t* name_off, char* out, uint64_t out_cap, uint64_t* out_used) { \
-        try { return NAME##_impl(ix, n, aln, mappings, mapping_pool_len, edits, edit_pool_len, n_reads, reads, quals, read_off, names, name_off, out, out_cap, out_used); } \
-        catch (...) { return GB_ERR_CAPACITY; }                                                                                    \
+        return gb::guarded(#NAME, [&] { return NAME##_impl(ix, n, aln, mappings, mapping_pool_len, edits, edit_pool_len, n_reads, reads, quals, \
+                                                           read_off, names, name_off, out, out_cap, out_used); });                  \
     }
 GB_EMIT_ENTRY(gb_emit_gaf)
 GB_EMIT_ENTRY(gb_emit_json)

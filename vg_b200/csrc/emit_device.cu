@@ -355,8 +355,6 @@ __global__ void emit_fill_kernel(EmitArgs A, const uint64_t* msg, const uint32_t
     }
 }
 
-inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 template <bool GAM>
 int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_mapping* d_mappings, uint64_t mapping_pool_len,
                 const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
@@ -374,19 +372,15 @@ int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_ma
     size_t scan64 = 0, scan32 = 0;
     GB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan64, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int64_t)m, d->stream));
     GB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan32, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int64_t)m, d->stream));
-    const size_t o_bytes = 256, o_framed = o_bytes + align256(8 * m), o_off = o_framed + (GAM ? align256(8 * m) : 0),
-                 o_present = o_off + align256(8 * m), o_pidx = o_present + (GAM ? align256(4 * m) : 0),
-                 o_tmp = o_pidx + (GAM ? align256(4 * m) : 0), ws_bytes = o_tmp + align256(std::max(scan64, scan32));
-    int rc;
-    if ((rc = d->emit_ws.reserve(ws_bytes))) return rc;
-    uint8_t* ws = d->emit_ws.ptr;
-    uint64_t* status = (uint64_t*)ws;
-    uint64_t* bytes = (uint64_t*)(ws + o_bytes);
-    uint64_t* framed = GAM ? (uint64_t*)(ws + o_framed) : bytes;
-    uint64_t* off = (uint64_t*)(ws + o_off);
-    uint32_t* present = GAM ? (uint32_t*)(ws + o_present) : nullptr;
-    uint32_t* pidx = GAM ? (uint32_t*)(ws + o_pidx) : nullptr;
-    void* tmp = ws + o_tmp;
+    size_t tb = std::max(scan64, scan32);
+    uint64_t *status, *bytes, *framed, *off;
+    uint32_t *present, *pidx;
+    void* tmp;
+    int rc = carve(d->emit_ws, [&](Carve& c) {
+        status = c.take<uint64_t>(2); bytes = c.take<uint64_t>(m); framed = GAM ? c.take<uint64_t>(m) : bytes; off = c.take<uint64_t>(m);
+        present = GAM ? c.take<uint32_t>(m) : nullptr; pidx = GAM ? c.take<uint32_t>(m) : nullptr; tmp = c.take<uint8_t>(tb);
+    });
+    if (rc) return rc;
 
     const uint32_t grid = (uint32_t)std::min<uint64_t>((m + EMIT_BLOCK - 1) / EMIT_BLOCK, (uint64_t)d->n_sms * 64);
     const uint32_t vgrid = (uint32_t)std::min<uint64_t>(((uint64_t)std::max(n, n_reads) + EMIT_BLOCK) / EMIT_BLOCK, (uint64_t)d->n_sms * 64);
@@ -395,13 +389,11 @@ int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_ma
     emit_size_kernel<GAM><<<grid, EMIT_BLOCK, 0, d->stream>>>(A, (const uint32_t*)status, bytes, present);
     d->launches += 2;
     GB_CUDA(cudaGetLastError());
-    size_t tb = align256(std::max(scan64, scan32));
     if (GAM) {
         GB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, present, pidx, (int64_t)m, d->stream));
         gam_frame_kernel<<<grid, EMIT_BLOCK, 0, d->stream>>>(n, bytes, pidx, framed);
         d->launches += 2;
         GB_CUDA(cudaGetLastError());
-        tb = align256(std::max(scan64, scan32));
     }
     GB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, framed, off, (int64_t)m, d->stream));
     d->launches++;
@@ -430,9 +422,8 @@ int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_ma
                         const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,  \
                         const uint64_t* d_read_off, const uint8_t* d_names, const uint64_t* d_name_off, char* d_out, uint64_t out_cap,        \
                         uint64_t* out_used) {                                                                                              \
-        try { return gb::emit_device<GAM>(dev, n, d_aln, d_mappings, mapping_pool_len, d_edits, edit_pool_len, n_reads, d_reads, d_quals, \
-                                          d_read_off, d_names, d_name_off, d_out, out_cap, out_used); }                                  \
-        catch (...) { return GB_ERR_CAPACITY; }                                                                                    \
+        return gb::guarded(#NAME, [&] { return gb::emit_device<GAM>(dev, n, d_aln, d_mappings, mapping_pool_len, d_edits, edit_pool_len, n_reads, \
+                                                                    d_reads, d_quals, d_read_off, d_names, d_name_off, d_out, out_cap, out_used); }); \
     }
 GB_EMIT_DEVICE_ENTRY(gb_emit_gaf_device, false)
 GB_EMIT_DEVICE_ENTRY(gb_emit_gam_device, true)

@@ -190,8 +190,6 @@ __global__ void __launch_bounds__(REC_WARPS * 32) fq_fill_kernel(Input in0, Inpu
     }
 }
 
-inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 int fastq_parse_device(gb_device* d, uint32_t n_inputs, const uint8_t* const* d_text, const uint64_t* text_bytes, uint32_t flags,
                        int final, uint32_t max_reads, uint8_t* d_reads, uint8_t* d_quals, uint64_t bases_cap, uint64_t* d_read_off,
                        uint8_t* d_names, uint64_t names_cap, uint64_t* d_name_off, uint32_t* n_reads, uint32_t* max_read_len,
@@ -221,44 +219,39 @@ int fastq_parse_device(gb_device* d, uint32_t n_inputs, const uint8_t* const* d_
     }
     GB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_reads, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int64_t)nr, d->stream));
     // workspace: summary, per input {tile counts, tile offsets, line ends}, per read {seq len, name len, error, offsets}, temp
-    size_t o = 256;
-    size_t o_tc[2], o_to[2], o_nl[2];
-    for (uint32_t t = 0; t < 2; t++) {
-        o_tc[t] = o; o += align256(8 * (n_tiles[t] + 1));
-        o_to[t] = o; o += align256(8 * (n_tiles[t] + 1));
-        o_nl[t] = o; o += t < n_inputs ? align256(8 * line_cap) : 0;
-    }
-    const size_t o_slen = o, o_nlen = o_slen + align256(8 * nr), o_err = o_nlen + align256(8 * nr), o_roff = o_err + align256(8 * nr),
-                 o_noff = o_roff + align256(8 * nr), o_tmp = o_noff + align256(8 * nr), ws_bytes = o_tmp + align256(std::max(scan_tiles, scan_reads));
-    int rc;
-    if ((rc = d->fastq_ws.reserve(ws_bytes))) return rc;
-    uint8_t* ws = d->fastq_ws.ptr;
-    FqSum* sum = (FqSum*)ws;
-    uint64_t *slen = (uint64_t*)(ws + o_slen), *nlen = (uint64_t*)(ws + o_nlen), *err = (uint64_t*)(ws + o_err),
-             *roff = (uint64_t*)(ws + o_roff), *noff = (uint64_t*)(ws + o_noff);
+    FqSum* sum;
+    uint64_t *tc[2], *to[2], *nl[2], *slen, *nlen, *err, *roff, *noff;
+    void* tmp;
+    int rc = carve(d->fastq_ws, [&](Carve& c) {
+        sum = c.take<FqSum>(1);
+        for (uint32_t t = 0; t < 2; t++) {
+            tc[t] = c.take<uint64_t>(n_tiles[t] + 1); to[t] = c.take<uint64_t>(n_tiles[t] + 1);
+            nl[t] = t < n_inputs ? c.take<uint64_t>(line_cap) : nullptr;
+        }
+        slen = c.take<uint64_t>(nr); nlen = c.take<uint64_t>(nr); err = c.take<uint64_t>(nr); roff = c.take<uint64_t>(nr); noff = c.take<uint64_t>(nr);
+        tmp = c.take<uint8_t>(std::max(scan_tiles, scan_reads));
+    });
+    if (rc) return rc;
     GB_CUDA(cudaMemsetAsync(sum, 0, sizeof(FqSum), d->stream));
     GB_CUDA(cudaMemsetAsync(&sum->first_bad, 0xff, sizeof(uint32_t), d->stream));
     GB_CUDA(cudaMemsetAsync(slen, 0, 8 * nr, d->stream));            // reads without a record scan as length 0
     GB_CUDA(cudaMemsetAsync(nlen, 0, 8 * nr, d->stream));
     Input in[2] = {};
     for (uint32_t t = 0; t < n_inputs; t++) {
-        in[t] = Input{d_text[t], text_bytes[t], (const uint64_t*)(ws + o_nl[t])};
-        uint64_t* tc = (uint64_t*)(ws + o_tc[t]);
-        uint64_t* to = (uint64_t*)(ws + o_to[t]);
+        in[t] = Input{d_text[t], text_bytes[t], nl[t]};
         const uintptr_t a0 = (uintptr_t)d_text[t] & ~(uintptr_t)15;
         const uint64_t n_vec = text_bytes[t] ? ((uintptr_t)d_text[t] + text_bytes[t] - a0 + 15) / 16 : 0;
-        GB_CUDA(cudaMemsetAsync(tc + n_tiles[t], 0, 8, d->stream));
+        GB_CUDA(cudaMemsetAsync(tc[t] + n_tiles[t], 0, 8, d->stream));
         if (n_tiles[t]) {
-            nl_count_kernel<<<(uint32_t)n_tiles[t], NL_THREADS, 0, d->stream>>>(d_text[t], text_bytes[t], a0, n_vec, tc);
+            nl_count_kernel<<<(uint32_t)n_tiles[t], NL_THREADS, 0, d->stream>>>(d_text[t], text_bytes[t], a0, n_vec, tc[t]);
             d->launches++;
             GB_CUDA(cudaGetLastError());
         }
-        GB_CUDA(cub::DeviceScan::ExclusiveSum(ws + o_tmp, scan_tiles, tc, to, (int64_t)(n_tiles[t] + 1), d->stream));
+        GB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_tiles, tc[t], to[t], (int64_t)(n_tiles[t] + 1), d->stream));
         d->launches++;
-        GB_CUDA(cudaMemcpyAsync(&sum->n_lines[t], to + n_tiles[t], 8, cudaMemcpyDeviceToDevice, d->stream));
+        GB_CUDA(cudaMemcpyAsync(&sum->n_lines[t], to[t] + n_tiles[t], 8, cudaMemcpyDeviceToDevice, d->stream));
         if (n_tiles[t]) {
-            nl_write_kernel<<<(uint32_t)n_tiles[t], NL_THREADS, 0, d->stream>>>(d_text[t], text_bytes[t], a0, n_vec, to, line_cap,
-                                                                               (uint64_t*)in[t].nl);
+            nl_write_kernel<<<(uint32_t)n_tiles[t], NL_THREADS, 0, d->stream>>>(d_text[t], text_bytes[t], a0, n_vec, to[t], line_cap, nl[t]);
             d->launches++;
             GB_CUDA(cudaGetLastError());
         }
@@ -267,8 +260,8 @@ int fastq_parse_device(gb_device* d, uint32_t n_inputs, const uint8_t* const* d_
         d->launches++;
         GB_CUDA(cudaGetLastError());
     }
-    GB_CUDA(cub::DeviceScan::ExclusiveSum(ws + o_tmp, scan_reads, slen, roff, (int64_t)nr, d->stream));
-    GB_CUDA(cub::DeviceScan::ExclusiveSum(ws + o_tmp, scan_reads, nlen, noff, (int64_t)nr, d->stream));
+    GB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_reads, slen, roff, (int64_t)nr, d->stream));
+    GB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_reads, nlen, noff, (int64_t)nr, d->stream));
     d->launches += 2;
     fq_finalize_kernel<<<1, 1, 0, d->stream>>>(in[0], in[1], mode, rec_cap, max_reads, bases_cap, names_cap, roff, noff, err, sum);
     const uint32_t rgrid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((nr + REC_WARPS - 1) / REC_WARPS, (uint64_t)d->n_sms * 8));
@@ -323,8 +316,8 @@ extern "C" int gb_fastq_parse_device(gb_device* dev, uint32_t n_inputs, const ui
                                      uint32_t flags, int final, uint32_t max_reads, uint8_t* d_reads, uint8_t* d_quals,
                                      uint64_t bases_cap, uint64_t* d_read_off, uint8_t* d_names, uint64_t names_cap,
                                      uint64_t* d_name_off, uint32_t* n_reads, uint32_t* max_read_len, uint64_t* text_used) {
-    try {
+    return gb::guarded("gb_fastq_parse_device", [&] {
         return gb::fastq_parse_device(dev, n_inputs, d_text, text_bytes, flags, final, max_reads, d_reads, d_quals, bases_cap,
                                       d_read_off, d_names, names_cap, d_name_off, n_reads, max_read_len, text_used);
-    } catch (...) { return GB_ERR_CAPACITY; }
+    });
 }

@@ -65,23 +65,25 @@ extern "C" int gb_sw_batch(gb_device* d, uint32_t n,
                            const uint32_t* node, const uint64_t* node_off, const uint32_t* pred, const uint64_t* pred_off,
                            const uint8_t* query, const uint64_t* query_off, uint32_t map_cap, uint32_t edit_cap,
                            int32_t* score, gb_mapping* maps, uint32_t* edits, uint32_t* n_maps, uint32_t* n_edits, uint8_t* status) {
-    if (!d || !node || !node_off || !pred || !pred_off || !query || !query_off || !score || !maps || !edits || !n_maps || !n_edits ||
-        !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
-    if (n == 0) return GB_OK;
-    GB_CUDA(cudaSetDevice(d->device));
-    DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
-    SeamOutBufs out;
-    DevBuf<int32_t> d_lastH, d_lastE; DevBuf<uint8_t> d_argH, d_argE; DevBuf<uint32_t> d_colstart, d_seqoff, d_seqlen;
-    SwBatch b;
-    int rc;
-    if ((rc = dag.validate(d, "gb_sw_batch")) || (rc = dag.check_limits("gb_sw_batch")) || (rc = dag.upload(d->stream, b.dag))) return rc;
-    const uint64_t cols = dag.col_off[n] + 1, nodes = dag.total_nodes + 1;
-    if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
-    if ((rc = d_lastH.reserve(cols)) || (rc = d_lastE.reserve(cols)) || (rc = d_argH.reserve(cols)) || (rc = d_argE.reserve(cols))) return rc;
-    if ((rc = d_colstart.reserve(nodes)) || (rc = d_seqoff.reserve(nodes)) || (rc = d_seqlen.reserve(nodes))) return rc;
-    b.out = out.view;
-    b.lastH = d_lastH.ptr; b.lastE = d_lastE.ptr; b.argH = d_argH.ptr; b.argE = d_argE.ptr;
-    b.col_start = d_colstart.ptr; b.seq_off = d_seqoff.ptr; b.seq_len = d_seqlen.ptr;
-    if ((rc = launch_warp_per_problem(d, sw_kernel, b, SW_WARPS, dp_smem_per_warp(dag.Lc) * SW_WARPS))) return rc;
-    return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+    return gb::guarded("gb_sw_batch", [&] {
+        if (!d || !node || !node_off || !pred || !pred_off || !query || !query_off || !score || !maps || !edits || !n_maps || !n_edits ||
+            !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
+        if (n == 0) return GB_OK;
+        GB_CUDA(cudaSetDevice(d->device));
+        DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
+        SeamOutBufs out;
+        DevBuf<int32_t> d_lastH, d_lastE; DevBuf<uint8_t> d_argH, d_argE; DevBuf<uint32_t> d_colstart, d_seqoff, d_seqlen;
+        SwBatch b;
+        int rc;
+        if ((rc = dag.validate(d, "gb_sw_batch")) || (rc = dag.check_limits("gb_sw_batch")) || (rc = dag.upload(d->stream, b.dag))) return rc;
+        const uint64_t cols = dag.col_off[n] + 1, nodes = dag.total_nodes + 1;
+        if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
+        if ((rc = d_lastH.reserve(cols)) || (rc = d_lastE.reserve(cols)) || (rc = d_argH.reserve(cols)) || (rc = d_argE.reserve(cols))) return rc;
+        if ((rc = d_colstart.reserve(nodes)) || (rc = d_seqoff.reserve(nodes)) || (rc = d_seqlen.reserve(nodes))) return rc;
+        b.out = out.view;
+        b.lastH = d_lastH.ptr; b.lastE = d_lastE.ptr; b.argH = d_argH.ptr; b.argE = d_argE.ptr;
+        b.col_start = d_colstart.ptr; b.seq_off = d_seqoff.ptr; b.seq_len = d_seqlen.ptr;
+        if ((rc = launch_warp_per_problem(d, sw_kernel, b, SW_WARPS, dp_smem_per_warp(dag.Lc) * SW_WARPS))) return rc;
+        return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+    });
 }

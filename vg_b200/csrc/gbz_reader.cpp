@@ -20,6 +20,7 @@
 //   GBWTGraph       tag 0x6B3764AF / version 3, nodes, flags, forward sequences (StringArray), node-to-segment translation
 // Only what this path needs is kept; anything the reader does not understand is GB_ERR_FORMAT, never a guess.
 #include "giraffe_b200.h"
+#include "entry_guard.h"
 
 #include <algorithm>
 #include <cstdio>
@@ -281,12 +282,11 @@ static int index_from_gbz_impl(const char* path, uint32_t k, uint32_t w, gb_host
 }
 
 extern "C" int gb_index_from_gbz(const char* path, uint32_t k, uint32_t w, gb_host_index** out) {
-    try { return index_from_gbz_impl(path, k, w, out); }          // no exception crosses the ABI
-    catch (...) { if (out) *out = nullptr; return GB_ERR_FORMAT; }
+    return gb::guarded("gb_index_from_gbz", GB_ERR_FORMAT, [&] { return index_from_gbz_impl(path, k, w, out); }, [&] { if (out) *out = nullptr; });
 }
 
 extern "C" int gb_index_from_gbz_min(const char* gbz_path, const char* min_path, const char* zipcodes_path, gb_host_index** out) {
-    try {
+    return gb::guarded("gb_index_from_gbz_min", GB_ERR_FORMAT, [&] {
         if (!gbz_path || !min_path || !out) return GB_ERR_ARG;
         *out = nullptr;
         MinFile m;
@@ -308,5 +308,5 @@ extern "C" int gb_index_from_gbz_min(const char* gbz_path, const char* min_path,
             if (oversized > n) return fail(".min points past the end of .zipcodes");
         }
         return index_from_gbz_impl(gbz_path, m.k, m.w, out, &m);
-    } catch (...) { if (out) *out = nullptr; return GB_ERR_FORMAT; }
+    }, [&] { if (out) *out = nullptr; });
 }

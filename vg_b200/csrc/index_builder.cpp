@@ -11,6 +11,7 @@
 // BASELINE.json configs and the reference's unit-test graphs can be loaded into HBM.
 
 #include "giraffe_b200.h"
+#include "entry_guard.h"
 #include "minimizer_common.h"
 
 #include <algorithm>
@@ -600,14 +601,11 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
     return GB_OK;
 }
 
-// No exception crosses the ABI: allocation failures and the like come back as status codes.
 extern "C" int gb_index_build(uint32_t n_node_ids, const uint8_t* node_seq, const uint64_t* node_off,
                               uint32_t n_paths, const uint32_t* path_nodes, const uint64_t* path_off,
                               const gb_dist_payload* dist, uint32_t k, uint32_t w,
                               gb_host_index** out) {
-    try { return index_build_impl(n_node_ids, node_seq, node_off, n_paths, path_nodes, path_off, dist, k, w, out); }
-    catch (const std::bad_alloc&) { return GB_ERR_CAPACITY; }
-    catch (...) { return GB_ERR_ARG; }
+    return gb::guarded("gb_index_build", [&] { return index_build_impl(n_node_ids, node_seq, node_off, n_paths, path_nodes, path_off, dist, k, w, out); });
 }
 
 extern "C" int gb_index_build_with_hits(uint32_t n_node_ids, const uint8_t* node_seq, const uint64_t* node_off,
@@ -617,9 +615,9 @@ extern "C" int gb_index_build_with_hits(uint32_t n_node_ids, const uint8_t* node
                                         gb_host_index** out) {
     static const uint64_t none = 0;
     if (n_hits == 0) { keys = keys ? keys : &none; positions = positions ? positions : &none; }
-    try { return index_build_impl(n_node_ids, node_seq, node_off, n_paths, path_nodes, path_off, dist, k, w, out, n_hits, keys, positions); }
-    catch (const std::bad_alloc&) { return GB_ERR_CAPACITY; }
-    catch (...) { return GB_ERR_ARG; }
+    return gb::guarded("gb_index_build_with_hits", [&] {
+        return index_build_impl(n_node_ids, node_seq, node_off, n_paths, path_nodes, path_off, dist, k, w, out, n_hits, keys, positions);
+    });
 }
 
 // The index from node sequences and a flat GBWT (the blob layout of gb_flat_index.gbwt) instead of haplotype paths: nothing here
@@ -628,7 +626,7 @@ extern "C" int gb_index_build_from_gbwt(uint32_t n_node_ids, const uint8_t* node
                                         const uint32_t* gbwt_words, uint64_t n_words, const uint32_t* rec_off,
                                         const gb_dist_payload* dist, uint32_t k, uint32_t w,
                                         uint64_t n_hits, const uint64_t* keys, const uint64_t* positions, gb_host_index** out) {
-    try {
+    return gb::guarded("gb_index_build_from_gbwt", [&] {
         if (!gbwt_words || !rec_off || !out || n_node_ids >= 0x7ffffff0u) return GB_ERR_ARG;
         const size_t n_nodes = 2 * ((size_t)n_node_ids + 1);
         std::vector<GbwtRecordIn> records(n_nodes);
@@ -646,9 +644,7 @@ extern "C" int gb_index_build_from_gbwt(uint32_t n_node_ids, const uint8_t* node
         const bool ext = keys || positions;
         if (ext && n_hits == 0) { keys = keys ? keys : &none; positions = positions ? positions : &none; }
         return index_build_impl(n_node_ids, node_seq, node_off, n_paths, nullptr, nullptr, dist, k, w, out, n_hits, keys, positions, &records);
-    }
-    catch (const std::bad_alloc&) { return GB_ERR_CAPACITY; }
-    catch (...) { return GB_ERR_ARG; }
+    });
 }
 
 extern "C" void gb_index_free(gb_host_index* ix) { delete ix; }
@@ -774,6 +770,5 @@ static int index_load_impl(const char* path, gb_host_index** out) {
 }
 
 extern "C" int gb_index_load(const char* path, gb_host_index** out) {
-    try { return index_load_impl(path, out); }
-    catch (...) { if (out) *out = nullptr; return GB_ERR_FORMAT; }
+    return gb::guarded("gb_index_load", GB_ERR_FORMAT, [&] { return index_load_impl(path, out); }, [&] { if (out) *out = nullptr; });
 }

@@ -697,14 +697,18 @@ extern "C" int gb_map_batch(gb_device* d, const gb_map_params* hp,
                             uint32_t n_reads, const uint8_t* reads, const uint8_t* quals, const uint64_t* read_off,
                             gb_alignment* aln, gb_mapping* mappings, uint64_t mapping_pool_cap, uint32_t* edits, uint64_t edit_pool_cap,
                             uint8_t* status, uint64_t* n_mappings_used, uint64_t* n_edits_used) {
-    return map_batch_host(d, hp, false, n_reads, reads, quals, read_off, aln, mappings, mapping_pool_cap, edits, edit_pool_cap, status, n_mappings_used, n_edits_used);
+    return gb::guarded("gb_map_batch", [&] {
+        return map_batch_host(d, hp, false, n_reads, reads, quals, read_off, aln, mappings, mapping_pool_cap, edits, edit_pool_cap, status, n_mappings_used, n_edits_used);
+    });
 }
 
 extern "C" int gb_map_paired_batch(gb_device* d, const gb_map_params* hp,
                                    uint32_t n_reads, const uint8_t* reads, const uint8_t* quals, const uint64_t* read_off,
                                    gb_alignment* aln, gb_mapping* mappings, uint64_t mapping_pool_cap, uint32_t* edits, uint64_t edit_pool_cap,
                                    uint8_t* status, uint64_t* n_mappings_used, uint64_t* n_edits_used) {
-    return map_batch_host(d, hp, true, n_reads, reads, quals, read_off, aln, mappings, mapping_pool_cap, edits, edit_pool_cap, status, n_mappings_used, n_edits_used);
+    return gb::guarded("gb_map_paired_batch", [&] {
+        return map_batch_host(d, hp, true, n_reads, reads, quals, read_off, aln, mappings, mapping_pool_cap, edits, edit_pool_cap, status, n_mappings_used, n_edits_used);
+    });
 }
 
 // Device-pointer entry: inputs already in HBM, outputs stay in HBM; asynchronous on the handle's stream.
@@ -712,11 +716,13 @@ extern "C" int gb_map_batch_device(gb_device* d, const gb_map_params* hp, int pa
                                    const uint8_t* d_reads, const uint8_t* d_quals, const uint64_t* d_read_off, uint32_t max_read_len,
                                    gb_alignment* d_aln, gb_mapping* d_mappings, uint64_t mapping_pool_cap, uint32_t* d_edits, uint64_t edit_pool_cap,
                                    uint8_t* d_status, uint64_t* d_totals) {
-    if (!d || !hp || !d_reads || !d_read_off || !d_aln || !d_mappings || !d_edits || !d_status || !d_totals) return GB_ERR_ARG;
-    if (n_reads == 0) return GB_OK;
-    GB_CUDA(cudaSetDevice(d->device));
-    return map_device(d, hp, n_reads, d_reads, d_quals, d_read_off, max_read_len, (uint64_t)n_reads * max_read_len, d_aln, d_status, paired != 0,
-                      d_mappings, mapping_pool_cap, d_edits, edit_pool_cap, nullptr, 0, d_totals, nullptr);
+    return gb::guarded("gb_map_batch_device", [&] {
+        if (!d || !hp || !d_reads || !d_read_off || !d_aln || !d_mappings || !d_edits || !d_status || !d_totals) return GB_ERR_ARG;
+        if (n_reads == 0) return GB_OK;
+        GB_CUDA(cudaSetDevice(d->device));
+        return map_device(d, hp, n_reads, d_reads, d_quals, d_read_off, max_read_len, (uint64_t)n_reads * max_read_len, d_aln, d_status, paired != 0,
+                          d_mappings, mapping_pool_cap, d_edits, edit_pool_cap, nullptr, 0, d_totals, nullptr);
+    });
 }
 
 // gb_map_batch_device cannot rerun a batch by itself (it only enqueues work): after synchronising, this tells whether the
@@ -742,7 +748,7 @@ extern "C" int gb_debug_seed_stage(gb_device* d, const gb_map_params* hp, int pa
                                    gb_seed* item_seeds, uint64_t item_seed_cap) {
     if (!d || !hp || !reads || !read_off || !out_reads || !mins || !seeds || !clusters || !items || !item_seeds) return GB_ERR_ARG;
     if (n_reads == 0) return GB_OK;
-    try {
+    return gb::guarded("gb_debug_seed_stage", [&] {
         GB_CUDA(cudaSetDevice(d->device));
         const uint64_t total = read_off[n_reads];
         uint32_t max_len = 0;
@@ -817,7 +823,7 @@ extern "C" int gb_debug_seed_stage(gb_device* d, const gb_map_params* hp, int pa
             nm += rs.min_cnt; ns += rs.seed_cnt; nc += rs.n_clusters; ni += rs.item_cnt;
         }
         return GB_OK;
-    } catch (...) { g_last_error = "stage dump: out of host memory"; return GB_ERR_CAPACITY; }
+    });
 }
 
 // Multi-GPU emission: gb_map_batch / gb_map_paired_batch additionally leave the records of the whole call in the caller's

@@ -141,105 +141,107 @@ extern "C" int gb_map_paired_job(gb_device* d, const gb_map_params* hp, gb_fragm
                                  uint32_t n_reads, const uint8_t* reads, const uint8_t* quals, const uint64_t* read_off,
                                  gb_alignment* aln, gb_mapping* mappings, uint64_t mapping_pool_cap, uint32_t* edits, uint64_t edit_pool_cap,
                                  uint8_t* status, uint8_t* pair_route, uint64_t* n_mappings_used, uint64_t* n_edits_used) {
-    if (!d || !hp || !f) { g_last_error = "gb_map_paired_job: null argument"; return GB_ERR_ARG; }
-    if (n_reads % 2 != 0) { g_last_error = "paired mapping needs an even number of reads"; return GB_ERR_ARG; }
-    if (hp->max_multimaps != 1) { g_last_error = "gb_map_paired_job reports one mapping per read (max_multimaps = 1); use gb_map_paired_batch with a forced distribution for multi-mapping"; return GB_ERR_ARG; }
-    if (training_window == 0) training_window = 2048;
-    const uint32_t n_pairs = n_reads / 2;
-    if (n_pairs == 0) { if (n_mappings_used) *n_mappings_used = 0; if (n_edits_used) *n_edits_used = 0; return GB_OK; }     // nothing to map: the distribution stays as it is
-    uint64_t nm = 0, ne = 0;
-    int rc;
-    std::vector<uint32_t> buffered;               // ambiguous_pair_buffer (pair indices)
-    uint32_t next = 0;                            // first pair not consumed yet
+    return gb::guarded("gb_map_paired_job", [&] {
+        if (!d || !hp || !f) { g_last_error = "gb_map_paired_job: null argument"; return GB_ERR_ARG; }
+        if (n_reads % 2 != 0) { g_last_error = "paired mapping needs an even number of reads"; return GB_ERR_ARG; }
+        if (hp->max_multimaps != 1) { g_last_error = "gb_map_paired_job reports one mapping per read (max_multimaps = 1); use gb_map_paired_batch with a forced distribution for multi-mapping"; return GB_ERR_ARG; }
+        if (training_window == 0) training_window = 2048;
+        const uint32_t n_pairs = n_reads / 2;
+        if (n_pairs == 0) { if (n_mappings_used) *n_mappings_used = 0; if (n_edits_used) *n_edits_used = 0; return GB_OK; }     // nothing to map: the distribution stays as it is
+        uint64_t nm = 0, ne = 0;
+        int rc;
+        std::vector<uint32_t> buffered;               // ambiguous_pair_buffer (pair indices)
+        uint32_t next = 0;                            // first pair not consumed yet
 
-    // ---- training: map(aln1), map(aln2), register unambiguous distances, in input order ------------------------
-    while (!f->is_fixed && next < n_pairs) {
-        const uint32_t wp = std::min(training_window, n_pairs - next), wr = 2 * wp;
-        const uint64_t base = read_off[2 * (uint64_t)next];
-        std::vector<uint64_t> off(wr + 1);
-        for (uint32_t i = 0; i <= wr; i++) off[i] = read_off[2 * (uint64_t)next + i] - base;
-        std::vector<gb_alignment> sa(wr); std::vector<uint8_t> ss(wr);
-        std::vector<gb_mapping> sm((size_t)wr * hp->mapping_cap_per_read); std::vector<uint32_t> se((size_t)wr * hp->edit_cap_per_read);
-        uint64_t um = 0, ue = 0;
-        if ((rc = gb_map_batch(d, hp, wr, reads + base, quals ? quals + base : nullptr, off.data(), sa.data(), sm.data(), sm.size(),
-                               se.data(), se.size(), ss.data(), &um, &ue))) return rc;
-        uint32_t consumed = 0;
-        for (uint32_t i = 0; i < wp && !f->is_fixed; i++, consumed++) {
-            const uint32_t pair = next + i;
-            bool both_perfect_unique = true;
-            for (uint32_t r = 0; r < 2; r++) {
-                const gb_alignment& a = sa[2 * i + r];
-                const int64_t L = (int64_t)(off[2 * i + r + 1] - off[2 * i + r]);
-                const double max_score_aln = (double)(d->sc.match * L);                      // score_exact_match (alignment_scorer.cpp:321)
-                both_perfect_unique = both_perfect_unique && ss[2 * i + r] == GB_ITEM_OK && (a.flags & GB_ALN_MAPPED) && a.mapq == 60 && (double)a.score >= max_score_aln * 0.85;
+        // ---- training: map(aln1), map(aln2), register unambiguous distances, in input order ------------------------
+        while (!f->is_fixed && next < n_pairs) {
+            const uint32_t wp = std::min(training_window, n_pairs - next), wr = 2 * wp;
+            const uint64_t base = read_off[2 * (uint64_t)next];
+            std::vector<uint64_t> off(wr + 1);
+            for (uint32_t i = 0; i <= wr; i++) off[i] = read_off[2 * (uint64_t)next + i] - base;
+            std::vector<gb_alignment> sa(wr); std::vector<uint8_t> ss(wr);
+            std::vector<gb_mapping> sm((size_t)wr * hp->mapping_cap_per_read); std::vector<uint32_t> se((size_t)wr * hp->edit_cap_per_read);
+            uint64_t um = 0, ue = 0;
+            if ((rc = gb_map_batch(d, hp, wr, reads + base, quals ? quals + base : nullptr, off.data(), sa.data(), sm.data(), sm.size(),
+                                   se.data(), se.size(), ss.data(), &um, &ue))) return rc;
+            uint32_t consumed = 0;
+            for (uint32_t i = 0; i < wp && !f->is_fixed; i++, consumed++) {
+                const uint32_t pair = next + i;
+                bool both_perfect_unique = true;
+                for (uint32_t r = 0; r < 2; r++) {
+                    const gb_alignment& a = sa[2 * i + r];
+                    const int64_t L = (int64_t)(off[2 * i + r + 1] - off[2 * i + r]);
+                    const double max_score_aln = (double)(d->sc.match * L);                      // score_exact_match (alignment_scorer.cpp:321)
+                    both_perfect_unique = both_perfect_unique && ss[2 * i + r] == GB_ITEM_OK && (a.flags & GB_ALN_MAPPED) && a.mapq == 60 && (double)a.score >= max_score_aln * 0.85;
+                }
+                bool keep = false;
+                if (both_perfect_unique) {
+                    // initial_position(aln1) -> final_position(reverse complement of aln2) = the flipped start of aln2
+                    const gb_mapping first1 = sm[sa[2 * i].mapping_off], first2 = sm[sa[2 * i + 1].mapping_off];
+                    const int64_t dist = host_oriented_distance(d, first1.node, first1.offset, first2.node ^ 1u,
+                                                                d->h_node_len[first2.node] - (uint32_t)first2.offset);
+                    if (!(dist == std::numeric_limits<int64_t>::max() || dist >= (int64_t)hp->max_fragment_length)) { f->add(dist); keep = true; }
+                }
+                if (keep) {
+                    for (uint32_t r = 0; r < 2; r++)
+                        // pair_all(mapped_pair) links the two single-ended records as mates (minimizer_mapper.cpp:1345-1350)
+                        if ((rc = append_records(sa.data(), sm.data(), se.data(), ss.data(), 2 * i + r, 2 * pair + r, GB_ALN_PAIRED, aln, mappings, mapping_pool_cap,
+                                                 edits, edit_pool_cap, status, nm, ne))) return rc;
+                    if (pair_route) pair_route[pair] = GB_PAIR_TRAINING;
+                } else {
+                    buffered.push_back(pair);
+                    if (pair_route) pair_route[pair] = GB_PAIR_BUFFERED;
+                }
             }
-            bool keep = false;
-            if (both_perfect_unique) {
-                // initial_position(aln1) -> final_position(reverse complement of aln2) = the flipped start of aln2
-                const gb_mapping first1 = sm[sa[2 * i].mapping_off], first2 = sm[sa[2 * i + 1].mapping_off];
-                const int64_t dist = host_oriented_distance(d, first1.node, first1.offset, first2.node ^ 1u,
-                                                            d->h_node_len[first2.node] - (uint32_t)first2.offset);
-                if (!(dist == std::numeric_limits<int64_t>::max() || dist >= (int64_t)hp->max_fragment_length)) { f->add(dist); keep = true; }
-            }
-            if (keep) {
-                for (uint32_t r = 0; r < 2; r++)
-                    // pair_all(mapped_pair) links the two single-ended records as mates (minimizer_mapper.cpp:1345-1350)
-                    if ((rc = append_records(sa.data(), sm.data(), se.data(), ss.data(), 2 * i + r, 2 * pair + r, GB_ALN_PAIRED, aln, mappings, mapping_pool_cap,
-                                             edits, edit_pool_cap, status, nm, ne))) return rc;
-                if (pair_route) pair_route[pair] = GB_PAIR_TRAINING;
-            } else {
-                buffered.push_back(pair);
-                if (pair_route) pair_route[pair] = GB_PAIR_BUFFERED;
-            }
+            next += consumed;
         }
-        next += consumed;
-    }
-    // end of input before the sample filled up: giraffe_main.cpp:2283-2296 finalizes with what there is
-    if (!f->is_fixed) f->is_fixed = true;
-    gb_map_params P = *hp;
-    P.fragment_mean = f->mu; P.fragment_stdev = f->sigma;
+        // end of input before the sample filled up: giraffe_main.cpp:2283-2296 finalizes with what there is
+        if (!f->is_fixed) f->is_fixed = true;
+        gb_map_params P = *hp;
+        P.fragment_mean = f->mu; P.fragment_stdev = f->sigma;
 
-    // ---- the remaining pairs, straight into the caller's pools ---------------------------------------------------
-    if (next < n_pairs) {
-        const uint32_t rr = 2 * (n_pairs - next);
-        const uint64_t base = read_off[2 * (uint64_t)next];
-        std::vector<uint64_t> off;
-        const uint64_t* off_p = read_off + 2 * (uint64_t)next;
-        if (base != 0) { off.resize(rr + 1); for (uint32_t i = 0; i <= rr; i++) off[i] = off_p[i] - base; off_p = off.data(); }
-        uint64_t um = 0, ue = 0;
-        if ((rc = gb_map_paired_batch(d, &P, rr, reads + base, quals ? quals + base : nullptr, off_p, aln + 2 * (size_t)next,
-                                      mappings + nm, mapping_pool_cap - nm, edits + ne, edit_pool_cap - ne, status + 2 * (size_t)next, &um, &ue))) return rc;
-        for (uint32_t i = 0; i < rr; i++) {
-            gb_alignment& a = aln[2 * (size_t)next + i];
-            a.read_id += 2 * next; a.mapping_off += (uint32_t)nm; a.edit_off += (uint32_t)ne;
+        // ---- the remaining pairs, straight into the caller's pools ---------------------------------------------------
+        if (next < n_pairs) {
+            const uint32_t rr = 2 * (n_pairs - next);
+            const uint64_t base = read_off[2 * (uint64_t)next];
+            std::vector<uint64_t> off;
+            const uint64_t* off_p = read_off + 2 * (uint64_t)next;
+            if (base != 0) { off.resize(rr + 1); for (uint32_t i = 0; i <= rr; i++) off[i] = off_p[i] - base; off_p = off.data(); }
+            uint64_t um = 0, ue = 0;
+            if ((rc = gb_map_paired_batch(d, &P, rr, reads + base, quals ? quals + base : nullptr, off_p, aln + 2 * (size_t)next,
+                                          mappings + nm, mapping_pool_cap - nm, edits + ne, edit_pool_cap - ne, status + 2 * (size_t)next, &um, &ue))) return rc;
+            for (uint32_t i = 0; i < rr; i++) {
+                gb_alignment& a = aln[2 * (size_t)next + i];
+                a.read_id += 2 * next; a.mapping_off += (uint32_t)nm; a.edit_off += (uint32_t)ne;
+            }
+            nm += um; ne += ue;
+            if (pair_route) for (uint32_t x = next; x < n_pairs; x++) pair_route[x] = GB_PAIR_PAIRED;
         }
-        nm += um; ne += ue;
-        if (pair_route) for (uint32_t x = next; x < n_pairs; x++) pair_route[x] = GB_PAIR_PAIRED;
-    }
-    // ---- the ambiguous buffer, mapped paired last (giraffe_main.cpp:2375-2396) -----------------------------------
-    if (!buffered.empty()) {
-        const uint32_t br = 2 * (uint32_t)buffered.size();
-        std::vector<uint64_t> off(br + 1, 0);
-        for (uint32_t i = 0; i < buffered.size(); i++) for (uint32_t r = 0; r < 2; r++) {
-            const uint64_t ri = 2 * (uint64_t)buffered[i] + r;
-            off[2 * i + r + 1] = off[2 * i + r] + (read_off[ri + 1] - read_off[ri]);
+        // ---- the ambiguous buffer, mapped paired last (giraffe_main.cpp:2375-2396) -----------------------------------
+        if (!buffered.empty()) {
+            const uint32_t br = 2 * (uint32_t)buffered.size();
+            std::vector<uint64_t> off(br + 1, 0);
+            for (uint32_t i = 0; i < buffered.size(); i++) for (uint32_t r = 0; r < 2; r++) {
+                const uint64_t ri = 2 * (uint64_t)buffered[i] + r;
+                off[2 * i + r + 1] = off[2 * i + r] + (read_off[ri + 1] - read_off[ri]);
+            }
+            std::vector<uint8_t> br_reads(off[br] + 16), br_quals(quals ? off[br] + 16 : 0);
+            for (uint32_t i = 0; i < buffered.size(); i++) for (uint32_t r = 0; r < 2; r++) {
+                const uint64_t ri = 2 * (uint64_t)buffered[i] + r, len = read_off[ri + 1] - read_off[ri];
+                memcpy(br_reads.data() + off[2 * i + r], reads + read_off[ri], len);
+                if (quals) memcpy(br_quals.data() + off[2 * i + r], quals + read_off[ri], len);
+            }
+            std::vector<gb_alignment> sa(br); std::vector<uint8_t> ss(br);
+            std::vector<gb_mapping> sm((size_t)br * hp->mapping_cap_per_read); std::vector<uint32_t> se((size_t)br * hp->edit_cap_per_read);
+            uint64_t um = 0, ue = 0;
+            if ((rc = gb_map_paired_batch(d, &P, br, br_reads.data(), quals ? br_quals.data() : nullptr, off.data(), sa.data(), sm.data(), sm.size(),
+                                          se.data(), se.size(), ss.data(), &um, &ue))) return rc;
+            for (uint32_t i = 0; i < buffered.size(); i++) for (uint32_t r = 0; r < 2; r++)
+                if ((rc = append_records(sa.data(), sm.data(), se.data(), ss.data(), 2 * i + r, 2 * buffered[i] + r, 0, aln, mappings, mapping_pool_cap,
+                                         edits, edit_pool_cap, status, nm, ne))) return rc;
         }
-        std::vector<uint8_t> br_reads(off[br] + 16), br_quals(quals ? off[br] + 16 : 0);
-        for (uint32_t i = 0; i < buffered.size(); i++) for (uint32_t r = 0; r < 2; r++) {
-            const uint64_t ri = 2 * (uint64_t)buffered[i] + r, len = read_off[ri + 1] - read_off[ri];
-            memcpy(br_reads.data() + off[2 * i + r], reads + read_off[ri], len);
-            if (quals) memcpy(br_quals.data() + off[2 * i + r], quals + read_off[ri], len);
-        }
-        std::vector<gb_alignment> sa(br); std::vector<uint8_t> ss(br);
-        std::vector<gb_mapping> sm((size_t)br * hp->mapping_cap_per_read); std::vector<uint32_t> se((size_t)br * hp->edit_cap_per_read);
-        uint64_t um = 0, ue = 0;
-        if ((rc = gb_map_paired_batch(d, &P, br, br_reads.data(), quals ? br_quals.data() : nullptr, off.data(), sa.data(), sm.data(), sm.size(),
-                                      se.data(), se.size(), ss.data(), &um, &ue))) return rc;
-        for (uint32_t i = 0; i < buffered.size(); i++) for (uint32_t r = 0; r < 2; r++)
-            if ((rc = append_records(sa.data(), sm.data(), se.data(), ss.data(), 2 * i + r, 2 * buffered[i] + r, 0, aln, mappings, mapping_pool_cap,
-                                     edits, edit_pool_cap, status, nm, ne))) return rc;
-    }
-    if (n_mappings_used) *n_mappings_used = nm;
-    if (n_edits_used) *n_edits_used = ne;
-    return GB_OK;
+        if (n_mappings_used) *n_mappings_used = nm;
+        if (n_edits_used) *n_edits_used = ne;
+        return GB_OK;
+    });
 }

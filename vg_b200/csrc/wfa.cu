@@ -561,52 +561,54 @@ extern "C" int gb_wfa_batch(gb_device* d, uint32_t n, const uint8_t* seq, const 
                             const uint32_t* pos, const double* error_model, uint32_t path_cap, uint32_t edit_cap,
                             int32_t* ok, int32_t* score, uint32_t* node_offset, uint32_t* seq_offset, uint32_t* length,
                             uint32_t* path, uint32_t* n_path, uint32_t* edits, uint32_t* n_edits) {
-    if (!d || !seq || !seq_off || !mode || !pos || !ok || !score || !node_offset || !seq_offset || !length || !path || !n_path ||
-        !edits || !n_edits || path_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
-    if (n == 0) return GB_OK;
-    GB_CUDA(cudaSetDevice(d->device));
-    static const double default_model[12] = {0.03, 1, 6, 0.05, 1, 10, 0.1, 1, 20, 0.1, 10, 200};     // gbwt_extender.hpp:372-381
-    const double* em = error_model ? error_model : default_model;
-    for (uint32_t i = 0; i < n; i++) {
-        if (mode[i] > 2) return GB_ERR_ARG;
-        if (seq_off[i + 1] - seq_off[i] > 60000) { g_last_error = "gb_wfa_batch: sequence too long"; return GB_ERR_ARG; }
-    }
-    const uint64_t total = seq_off[n];
-    const uint32_t grid = std::max<uint32_t>(1u, std::min<uint32_t>((uint32_t)d->n_sms * 4, (n + WFA_THREADS - 1) / WFA_THREADS));
-    const size_t threads = (size_t)grid * WFA_THREADS;
-    DevBuf<uint8_t> d_seq, d_work, d_pool; DevBuf<uint64_t> d_soff, d_hash; DevBuf<uint32_t> d_mode, d_pos, d_noff, d_sqoff, d_len, d_np, d_ne, d_path, d_edits, d_ppool, d_counter;
-    DevBuf<int32_t> d_ok, d_score; DevBuf<double> d_em; DevBuf<WfaNode> d_nodes; DevBuf<WfaScore> d_scores;
-    int rc;
-    if ((rc = d_seq.upload(seq, total ? total : 1, d->stream, total)) || (rc = d_work.reserve(total ? total : 1))) return rc;
-    if ((rc = d_soff.upload(seq_off, n + 1, d->stream)) || (rc = d_mode.upload(mode, n, d->stream)) || (rc = d_pos.upload(pos, 4 * (size_t)n, d->stream))) return rc;
-    if ((rc = d_em.upload(em, 12, d->stream))) return rc;
-    if ((rc = d_ok.reserve(n)) || (rc = d_score.reserve(n)) || (rc = d_noff.reserve(n)) || (rc = d_sqoff.reserve(n)) || (rc = d_len.reserve(n)) ||
-        (rc = d_np.reserve(n)) || (rc = d_ne.reserve(n))) return rc;
-    if ((rc = d_path.reserve((size_t)n * path_cap)) || (rc = d_edits.reserve((size_t)n * edit_cap))) return rc;
-    if ((rc = d_nodes.reserve(threads * WFA_NODES)) || (rc = d_pool.reserve(threads * WFA_SEQ_POOL)) || (rc = d_ppool.reserve(threads * WFA_PATH_POOL)) ||
-        (rc = d_hash.reserve(threads * WFA_HASH)) || (rc = d_scores.reserve(threads * WFA_SCORES)) || (rc = d_counter.reserve(4))) return rc;
-    GB_CUDA(cudaMemsetAsync(d_counter.ptr, 0, 16, d->stream));
-    WfaBatch b;
-    b.n = n; b.seq = d_seq.ptr; b.seq_off = d_soff.ptr; b.mode = d_mode.ptr; b.pos = d_pos.ptr; b.error_model = d_em.ptr;
-    b.ok = d_ok.ptr; b.score = d_score.ptr; b.node_offset = d_noff.ptr; b.seq_offset = d_sqoff.ptr; b.length = d_len.ptr; b.n_path = d_np.ptr; b.n_edits = d_ne.ptr;
-    b.path = d_path.ptr; b.edits = d_edits.ptr; b.path_cap = path_cap; b.edit_cap = edit_cap; b.work_seq = d_work.ptr;
-    b.nodes = d_nodes.ptr; b.seq_pool = d_pool.ptr; b.path_pool = d_ppool.ptr; b.hash = d_hash.ptr; b.scores = d_scores.ptr; b.work_counter = d_counter.ptr;
-    { const char* env = std::getenv("GIRAFFE_B200_WFA_SMALL_TABLE"); b.first_hash_mask = (env && std::atoi(env) == 0) ? WFA_HASH - 1 : WFA_HASH_SMALL - 1; }
-    GB_CUDA(cudaEventRecord(d->ev0, d->stream));
-    wfa_kernel<<<grid, WFA_THREADS, 0, d->stream>>>(d->ix, d->sc, b);
-    d->launches++;
-    GB_CUDA(cudaGetLastError());
-    GB_CUDA(cudaEventRecord(d->ev1, d->stream));
-    GB_CUDA(cudaMemcpyAsync(ok, d_ok.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(score, d_score.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(node_offset, d_noff.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(seq_offset, d_sqoff.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(length, d_len.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(n_path, d_np.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(n_edits, d_ne.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(path, d_path.ptr, 4 * (size_t)n * path_cap, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaMemcpyAsync(edits, d_edits.ptr, 4 * (size_t)n * edit_cap, cudaMemcpyDeviceToHost, d->stream));
-    GB_CUDA(cudaStreamSynchronize(d->stream));
-    GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
-    return GB_OK;
+    return gb::guarded("gb_wfa_batch", [&] {
+        if (!d || !seq || !seq_off || !mode || !pos || !ok || !score || !node_offset || !seq_offset || !length || !path || !n_path ||
+            !edits || !n_edits || path_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
+        if (n == 0) return GB_OK;
+        GB_CUDA(cudaSetDevice(d->device));
+        static const double default_model[12] = {0.03, 1, 6, 0.05, 1, 10, 0.1, 1, 20, 0.1, 10, 200};     // gbwt_extender.hpp:372-381
+        const double* em = error_model ? error_model : default_model;
+        for (uint32_t i = 0; i < n; i++) {
+            if (mode[i] > 2) return GB_ERR_ARG;
+            if (seq_off[i + 1] - seq_off[i] > 60000) { g_last_error = "gb_wfa_batch: sequence too long"; return GB_ERR_ARG; }
+        }
+        const uint64_t total = seq_off[n];
+        const uint32_t grid = std::max<uint32_t>(1u, std::min<uint32_t>((uint32_t)d->n_sms * 4, (n + WFA_THREADS - 1) / WFA_THREADS));
+        const size_t threads = (size_t)grid * WFA_THREADS;
+        DevBuf<uint8_t> d_seq, d_work, d_pool; DevBuf<uint64_t> d_soff, d_hash; DevBuf<uint32_t> d_mode, d_pos, d_noff, d_sqoff, d_len, d_np, d_ne, d_path, d_edits, d_ppool, d_counter;
+        DevBuf<int32_t> d_ok, d_score; DevBuf<double> d_em; DevBuf<WfaNode> d_nodes; DevBuf<WfaScore> d_scores;
+        int rc;
+        if ((rc = d_seq.upload(seq, total ? total : 1, d->stream, total)) || (rc = d_work.reserve(total ? total : 1))) return rc;
+        if ((rc = d_soff.upload(seq_off, n + 1, d->stream)) || (rc = d_mode.upload(mode, n, d->stream)) || (rc = d_pos.upload(pos, 4 * (size_t)n, d->stream))) return rc;
+        if ((rc = d_em.upload(em, 12, d->stream))) return rc;
+        if ((rc = d_ok.reserve(n)) || (rc = d_score.reserve(n)) || (rc = d_noff.reserve(n)) || (rc = d_sqoff.reserve(n)) || (rc = d_len.reserve(n)) ||
+            (rc = d_np.reserve(n)) || (rc = d_ne.reserve(n))) return rc;
+        if ((rc = d_path.reserve((size_t)n * path_cap)) || (rc = d_edits.reserve((size_t)n * edit_cap))) return rc;
+        if ((rc = d_nodes.reserve(threads * WFA_NODES)) || (rc = d_pool.reserve(threads * WFA_SEQ_POOL)) || (rc = d_ppool.reserve(threads * WFA_PATH_POOL)) ||
+            (rc = d_hash.reserve(threads * WFA_HASH)) || (rc = d_scores.reserve(threads * WFA_SCORES)) || (rc = d_counter.reserve(4))) return rc;
+        GB_CUDA(cudaMemsetAsync(d_counter.ptr, 0, 16, d->stream));
+        WfaBatch b;
+        b.n = n; b.seq = d_seq.ptr; b.seq_off = d_soff.ptr; b.mode = d_mode.ptr; b.pos = d_pos.ptr; b.error_model = d_em.ptr;
+        b.ok = d_ok.ptr; b.score = d_score.ptr; b.node_offset = d_noff.ptr; b.seq_offset = d_sqoff.ptr; b.length = d_len.ptr; b.n_path = d_np.ptr; b.n_edits = d_ne.ptr;
+        b.path = d_path.ptr; b.edits = d_edits.ptr; b.path_cap = path_cap; b.edit_cap = edit_cap; b.work_seq = d_work.ptr;
+        b.nodes = d_nodes.ptr; b.seq_pool = d_pool.ptr; b.path_pool = d_ppool.ptr; b.hash = d_hash.ptr; b.scores = d_scores.ptr; b.work_counter = d_counter.ptr;
+        { const char* env = std::getenv("GIRAFFE_B200_WFA_SMALL_TABLE"); b.first_hash_mask = (env && std::atoi(env) == 0) ? WFA_HASH - 1 : WFA_HASH_SMALL - 1; }
+        GB_CUDA(cudaEventRecord(d->ev0, d->stream));
+        wfa_kernel<<<grid, WFA_THREADS, 0, d->stream>>>(d->ix, d->sc, b);
+        d->launches++;
+        GB_CUDA(cudaGetLastError());
+        GB_CUDA(cudaEventRecord(d->ev1, d->stream));
+        GB_CUDA(cudaMemcpyAsync(ok, d_ok.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(score, d_score.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(node_offset, d_noff.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(seq_offset, d_sqoff.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(length, d_len.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(n_path, d_np.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(n_edits, d_ne.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(path, d_path.ptr, 4 * (size_t)n * path_cap, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaMemcpyAsync(edits, d_edits.ptr, 4 * (size_t)n * edit_cap, cudaMemcpyDeviceToHost, d->stream));
+        GB_CUDA(cudaStreamSynchronize(d->stream));
+        GB_CUDA(cudaEventElapsedTime(&d->last_kernel_ms, d->ev0, d->ev1));
+        return GB_OK;
+    });
 }

@@ -69,56 +69,58 @@ extern "C" int gb_xdrop_dag_batch(gb_device* d, uint32_t n,
                                   const uint8_t* query, const uint64_t* query_off, const uint32_t* seed, const uint32_t* max_gap,
                                   uint32_t map_cap, uint32_t edit_cap,
                                   int32_t* score, gb_mapping* maps, uint32_t* edits, uint32_t* n_maps, uint32_t* n_edits, uint8_t* status) {
-    if (!d || !node || !node_off || !pred || !pred_off || !query || !query_off || !seed || !max_gap || !score || !maps || !edits ||
-        !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
-    if (n == 0) return GB_OK;
-    GB_CUDA(cudaSetDevice(d->device));
-    DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
-    int rc;
-    if ((rc = dag.validate(d, "gb_xdrop_dag_batch"))) return rc;
-    for (uint32_t p = 0; p < n; p++) {
-        // vg's max_gap is a uint16_t (DozeuInterface::align), and the X-drop threshold go + ge * (max_gap - 1) is int32
-        if (max_gap[p] > 65535) return DagProblems::fail("gb_xdrop_dag_batch", ": max_gap above 65535");
-        // a seed lies in its problem: a node of the list, an offset up to that node's length, a query offset up to m
-        const uint32_t su = seed[3 * p], so = seed[3 * p + 1], sq = seed[3 * p + 2];
-        if (su == 0xffffffffu) continue;
-        if (su >= dag.N[p]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed node outside the problem");
-        if (so > d->h_node_len[node[node_off[p] + su]]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed offset past the seed node");
-        if (sq > dag.m[p]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed query offset past the query");
-    }
-    // successor CSR, ascending (nodes are visited in ascending order), at most 255 successors per node
-    const uint64_t total_pred = pred_off[dag.total_nodes];
-    std::vector<uint64_t> succ_off(dag.total_nodes + 1, 0);
-    std::vector<uint32_t> succ(total_pred ? total_pred : 1);
-    for (uint32_t p = 0; p < n; p++) {
-        const uint64_t n0 = node_off[p], N = dag.N[p];
-        std::vector<uint32_t> deg(N, 0);
-        for (uint64_t e = pred_off[n0]; e < pred_off[n0 + N]; e++) deg[pred[e]]++;
-        for (uint64_t u = 0; u < N; u++) {
-            if (deg[u] > 255) { g_last_error = "gb_xdrop_dag_batch: more than 255 successors"; return GB_ERR_ARG; }
-            succ_off[n0 + u + 1] = succ_off[n0 + u] + deg[u];
+    return gb::guarded("gb_xdrop_dag_batch", [&] {
+        if (!d || !node || !node_off || !pred || !pred_off || !query || !query_off || !seed || !max_gap || !score || !maps || !edits ||
+            !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
+        if (n == 0) return GB_OK;
+        GB_CUDA(cudaSetDevice(d->device));
+        DagProblems dag(n, node, node_off, pred, pred_off, query, query_off);
+        int rc;
+        if ((rc = dag.validate(d, "gb_xdrop_dag_batch"))) return rc;
+        for (uint32_t p = 0; p < n; p++) {
+            // vg's max_gap is a uint16_t (DozeuInterface::align), and the X-drop threshold go + ge * (max_gap - 1) is int32
+            if (max_gap[p] > 65535) return DagProblems::fail("gb_xdrop_dag_batch", ": max_gap above 65535");
+            // a seed lies in its problem: a node of the list, an offset up to that node's length, a query offset up to m
+            const uint32_t su = seed[3 * p], so = seed[3 * p + 1], sq = seed[3 * p + 2];
+            if (su == 0xffffffffu) continue;
+            if (su >= dag.N[p]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed node outside the problem");
+            if (so > d->h_node_len[node[node_off[p] + su]]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed offset past the seed node");
+            if (sq > dag.m[p]) return DagProblems::fail("gb_xdrop_dag_batch", ": seed query offset past the query");
         }
-        std::vector<uint32_t> fill(N, 0);
-        for (uint64_t u = 0; u < N; u++)
-            for (uint64_t e = pred_off[n0 + u]; e < pred_off[n0 + u + 1]; e++) { const uint32_t pu = pred[e]; succ[succ_off[n0 + pu] + fill[pu]++] = (uint32_t)u; }
-    }
-    XdBatch b;
-    if ((rc = dag.check_limits("gb_xdrop_dag_batch")) || (rc = dag.upload(d->stream, b.dag))) return rc;
-    SeamOutBufs out;
-    DevBuf<uint32_t> d_succ, d_seed, d_gap, d_colstart, d_seqoff, d_seqlen; DevBuf<uint64_t> d_soff;
-    DevBuf<int32_t> d_lastH, d_lastE; DevBuf<uint8_t> d_argH, d_argE; DevBuf<XdNode> d_nstate;
-    const uint64_t cols = dag.col_off[n] + 1, nodes = dag.total_nodes + 1;
-    if ((rc = d_succ.upload(succ.data(), total_pred ? total_pred : 1, d->stream, total_pred))) return rc;
-    if ((rc = d_soff.upload(succ_off.data(), dag.total_nodes + 1, d->stream))) return rc;
-    if ((rc = d_seed.upload(seed, 3 * (size_t)n, d->stream))) return rc;
-    if ((rc = d_gap.upload(max_gap, n, d->stream))) return rc;
-    if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
-    if ((rc = d_lastH.reserve(cols)) || (rc = d_lastE.reserve(cols)) || (rc = d_argH.reserve(cols)) || (rc = d_argE.reserve(cols))) return rc;
-    if ((rc = d_colstart.reserve(nodes)) || (rc = d_seqoff.reserve(nodes)) || (rc = d_seqlen.reserve(nodes)) || (rc = d_nstate.reserve(nodes))) return rc;
-    b.out = out.view;
-    b.succ = d_succ.ptr; b.succ_off = d_soff.ptr; b.seed = d_seed.ptr; b.max_gap = d_gap.ptr;
-    b.lastH = d_lastH.ptr; b.lastE = d_lastE.ptr; b.argH = d_argH.ptr; b.argE = d_argE.ptr;
-    b.col_start = d_colstart.ptr; b.seq_off = d_seqoff.ptr; b.seq_len = d_seqlen.ptr; b.nstate = d_nstate.ptr;
-    if ((rc = launch_warp_per_problem(d, xdrop_dag_kernel, b, XD_WARPS, dp_smem_per_warp(dag.Lc) * XD_WARPS))) return rc;
-    return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+        // successor CSR, ascending (nodes are visited in ascending order), at most 255 successors per node
+        const uint64_t total_pred = pred_off[dag.total_nodes];
+        std::vector<uint64_t> succ_off(dag.total_nodes + 1, 0);
+        std::vector<uint32_t> succ(total_pred ? total_pred : 1);
+        for (uint32_t p = 0; p < n; p++) {
+            const uint64_t n0 = node_off[p], N = dag.N[p];
+            std::vector<uint32_t> deg(N, 0);
+            for (uint64_t e = pred_off[n0]; e < pred_off[n0 + N]; e++) deg[pred[e]]++;
+            for (uint64_t u = 0; u < N; u++) {
+                if (deg[u] > 255) { g_last_error = "gb_xdrop_dag_batch: more than 255 successors"; return GB_ERR_ARG; }
+                succ_off[n0 + u + 1] = succ_off[n0 + u] + deg[u];
+            }
+            std::vector<uint32_t> fill(N, 0);
+            for (uint64_t u = 0; u < N; u++)
+                for (uint64_t e = pred_off[n0 + u]; e < pred_off[n0 + u + 1]; e++) { const uint32_t pu = pred[e]; succ[succ_off[n0 + pu] + fill[pu]++] = (uint32_t)u; }
+        }
+        XdBatch b;
+        if ((rc = dag.check_limits("gb_xdrop_dag_batch")) || (rc = dag.upload(d->stream, b.dag))) return rc;
+        SeamOutBufs out;
+        DevBuf<uint32_t> d_succ, d_seed, d_gap, d_colstart, d_seqoff, d_seqlen; DevBuf<uint64_t> d_soff;
+        DevBuf<int32_t> d_lastH, d_lastE; DevBuf<uint8_t> d_argH, d_argE; DevBuf<XdNode> d_nstate;
+        const uint64_t cols = dag.col_off[n] + 1, nodes = dag.total_nodes + 1;
+        if ((rc = d_succ.upload(succ.data(), total_pred ? total_pred : 1, d->stream, total_pred))) return rc;
+        if ((rc = d_soff.upload(succ_off.data(), dag.total_nodes + 1, d->stream))) return rc;
+        if ((rc = d_seed.upload(seed, 3 * (size_t)n, d->stream))) return rc;
+        if ((rc = d_gap.upload(max_gap, n, d->stream))) return rc;
+        if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
+        if ((rc = d_lastH.reserve(cols)) || (rc = d_lastE.reserve(cols)) || (rc = d_argH.reserve(cols)) || (rc = d_argE.reserve(cols))) return rc;
+        if ((rc = d_colstart.reserve(nodes)) || (rc = d_seqoff.reserve(nodes)) || (rc = d_seqlen.reserve(nodes)) || (rc = d_nstate.reserve(nodes))) return rc;
+        b.out = out.view;
+        b.succ = d_succ.ptr; b.succ_off = d_soff.ptr; b.seed = d_seed.ptr; b.max_gap = d_gap.ptr;
+        b.lastH = d_lastH.ptr; b.lastE = d_lastE.ptr; b.argH = d_argH.ptr; b.argE = d_argE.ptr;
+        b.col_start = d_colstart.ptr; b.seq_off = d_seqoff.ptr; b.seq_len = d_seqlen.ptr; b.nstate = d_nstate.ptr;
+        if ((rc = launch_warp_per_problem(d, xdrop_dag_kernel, b, XD_WARPS, dp_smem_per_warp(dag.Lc) * XD_WARPS))) return rc;
+        return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+    });
 }

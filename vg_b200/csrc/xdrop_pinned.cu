@@ -154,107 +154,109 @@ extern "C" int gb_xdrop_pinned_batch(gb_device* d, uint32_t n,
                                      const uint32_t* max_gap, uint32_t map_cap, uint32_t edit_cap,
                                      int32_t* score, gb_mapping* maps, uint32_t* edits, uint32_t* n_maps, uint32_t* n_edits,
                                      uint8_t* status) {
-    if (!d || !tree_parent || !tree_node || !tree_off || !root_trim || !query || !query_off || !max_gap || !score || !maps ||
-        !edits || !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
-    if (n == 0) return GB_OK;
-    // ---- validation, before anything reaches the device: known nodes; one root, first; the nodes in DFS visit order (both
-    // kernels keep one DP column per tree level, which a node's parent must still own); the root trim leaves a base; fewer
-    // than TAIL_D_CAP levels ----
-    std::vector<uint64_t> prob_bases(n, 0); std::vector<uint32_t> prob_depth(n, 0), lineage;
-    uint32_t max_q = 0, Lc;
-    auto fail = [](const char* what) { g_last_error = std::string("gb_xdrop_pinned_batch: ") + what; return GB_ERR_ARG; };
-    for (uint32_t i = 0; i < n; i++) {
-        max_q = std::max<uint32_t>(max_q, (uint32_t)(query_off[i + 1] - query_off[i]));
-        const uint64_t t0 = tree_off[i]; const uint32_t ntree = (uint32_t)(tree_off[i + 1] - t0);
-        if (ntree == 0) return fail("empty tree");
-        if (max_gap[i] > 65535) return fail("max_gap above 65535");      // vg's max_gap is a uint16_t
-        lineage.clear();                     // root .. previous node
-        for (uint32_t x = 0; x < ntree; x++) {
-            const uint32_t v = tree_node[t0 + x]; const int32_t par = tree_parent[t0 + x];
-            if (v < 2 || v >= d->ix.n_nodes || d->h_node_len[v] == 0) return fail("unknown node");
-            if (x == 0 && par >= 0) return fail("the first tree node is not a root");
-            if (x > 0 && par < 0) return fail("more than one root");
-            if (par >= (int32_t)x) return fail("a parent does not precede its child");
-            while (par >= 0 && !lineage.empty() && lineage.back() != (uint32_t)par) lineage.pop_back();
-            if (par >= 0 && lineage.empty()) return fail("tree nodes are not in DFS visit order");
-            lineage.push_back(x);
-            const uint32_t len = d->h_node_len[v];
-            if (par < 0) {
-                if (root_trim[i] >= len) return fail("root_trim leaves no base of the root");
-                prob_bases[i] += len - root_trim[i];
-            } else prob_bases[i] += len;
-            if (lineage.size() > TAIL_D_CAP) return fail("tree deeper than 511 levels");
-            prob_depth[i] = std::max<uint32_t>(prob_depth[i], (uint32_t)lineage.size() - 1);
-        }
-    }
-    int rc;
-    if ((rc = query_columns(max_q, Lc))) return rc;
-    GB_CUDA(cudaSetDevice(d->device));
-    DevBuf<int32_t> d_par; DevBuf<uint32_t> d_node, d_trim, d_gap, d_counter; DevBuf<uint64_t> d_toff, d_qoff;
-    DevBuf<uint8_t> d_q, d_ws; SeamOutBufs out;
-    const uint64_t nt = tree_off[n], nq = query_off[n];
-    if ((rc = d_par.upload(tree_parent, nt ? nt : 1, d->stream, nt))) return rc;
-    if ((rc = d_node.upload(tree_node, nt ? nt : 1, d->stream, nt))) return rc;
-    if ((rc = d_toff.upload(tree_off, n + 1, d->stream))) return rc;
-    if ((rc = d_trim.upload(root_trim, n, d->stream))) return rc;
-    if ((rc = d_gap.upload(max_gap, n, d->stream))) return rc;
-    if ((rc = d_q.upload(query, nq ? nq : 1, d->stream, nq))) return rc;
-    if ((rc = d_qoff.upload(query_off, n + 1, d->stream))) return rc;
-    if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
-    if ((rc = d_counter.reserve(4))) return rc;
-    GB_CUDA(cudaMemsetAsync(d_counter.ptr, 0, 16, d->stream));
-    const size_t smem = dp_smem_per_warp(Lc) * XP_WARPS;
-    if (smem > 48 * 1024) GB_CUDA(cudaFuncSetAttribute(xdrop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    uint32_t grid = std::min<uint32_t>((uint32_t)d->n_sms * 2, (n + XP_WARPS - 1) / XP_WARPS);
-    const uint32_t tb_cells = 2 * 1024 * 1024;
-    const size_t ws_stride = tail_ws_bytes(Lc, tb_cells);
-    if ((rc = d_ws.reserve(ws_stride * grid * XP_WARPS))) return rc;
-    XdropBatch b;
-    b.tree_parent = d_par.ptr; b.tree_node = d_node.ptr; b.tree_off = d_toff.ptr; b.root_trim = d_trim.ptr;
-    b.query = d_q.ptr; b.query_off = d_qoff.ptr; b.max_gap = d_gap.ptr; b.n = n; b.Lc = Lc; b.out = out.view;
-    b.ws_base = d_ws.ptr; b.ws_stride = ws_stride; b.tb_cells = tb_cells;
-    b.work_counter = d_counter.ptr;
-    // ---- problems the int16 tile kernel can hold run there (the production path of the tails); the rest on the int32 sweep ----
-    std::vector<uint8_t> elig(n, 0); std::vector<uint32_t> toff(n, 0);
-    uint64_t units = 0; uint32_t n_elig = 0;
-    if (d->use_tiles) {
+    return gb::guarded("gb_xdrop_pinned_batch", [&] {
+        if (!d || !tree_parent || !tree_node || !tree_off || !root_trim || !query || !query_off || !max_gap || !score || !maps ||
+            !edits || !n_maps || !n_edits || !status || map_cap == 0 || edit_cap == 0) return GB_ERR_ARG;
+        if (n == 0) return GB_OK;
+        // ---- validation, before anything reaches the device: known nodes; one root, first; the nodes in DFS visit order (both
+        // kernels keep one DP column per tree level, which a node's parent must still own); the root trim leaves a base; fewer
+        // than TAIL_D_CAP levels ----
+        std::vector<uint64_t> prob_bases(n, 0); std::vector<uint32_t> prob_depth(n, 0), lineage;
+        uint32_t max_q = 0, Lc;
+        auto fail = [](const char* what) { g_last_error = std::string("gb_xdrop_pinned_batch: ") + what; return GB_ERR_ARG; };
         for (uint32_t i = 0; i < n; i++) {
-            const uint32_t ntree = (uint32_t)(tree_off[i + 1] - tree_off[i]), m = (uint32_t)(query_off[i + 1] - query_off[i]);
-            const uint32_t bases = (uint32_t)std::min<uint64_t>(prob_bases[i], 0xffffffffu);
-            if (!tile_eligible(d->sc, m, std::max(max_gap[i], 1u), ntree, bases, prob_depth[i])) continue;
-            elig[i] = 1; toff[i] = (uint32_t)units; units += tile_bytes(ntree, bases, m) / 16; n_elig++;
+            max_q = std::max<uint32_t>(max_q, (uint32_t)(query_off[i + 1] - query_off[i]));
+            const uint64_t t0 = tree_off[i]; const uint32_t ntree = (uint32_t)(tree_off[i + 1] - t0);
+            if (ntree == 0) return fail("empty tree");
+            if (max_gap[i] > 65535) return fail("max_gap above 65535");      // vg's max_gap is a uint16_t
+            lineage.clear();                     // root .. previous node
+            for (uint32_t x = 0; x < ntree; x++) {
+                const uint32_t v = tree_node[t0 + x]; const int32_t par = tree_parent[t0 + x];
+                if (v < 2 || v >= d->ix.n_nodes || d->h_node_len[v] == 0) return fail("unknown node");
+                if (x == 0 && par >= 0) return fail("the first tree node is not a root");
+                if (x > 0 && par < 0) return fail("more than one root");
+                if (par >= (int32_t)x) return fail("a parent does not precede its child");
+                while (par >= 0 && !lineage.empty() && lineage.back() != (uint32_t)par) lineage.pop_back();
+                if (par >= 0 && lineage.empty()) return fail("tree nodes are not in DFS visit order");
+                lineage.push_back(x);
+                const uint32_t len = d->h_node_len[v];
+                if (par < 0) {
+                    if (root_trim[i] >= len) return fail("root_trim leaves no base of the root");
+                    prob_bases[i] += len - root_trim[i];
+                } else prob_bases[i] += len;
+                if (lineage.size() > TAIL_D_CAP) return fail("tree deeper than 511 levels");
+                prob_depth[i] = std::max<uint32_t>(prob_depth[i], (uint32_t)lineage.size() - 1);
+            }
         }
-    }
-    DevBuf<uint8_t> d_elig, d_tiles; DevBuf<uint32_t> d_tileoff, d_lists, d_paths; DevBuf<TileCounters> d_tc; DevBuf<TileResult> d_res;
-    GB_CUDA(cudaEventRecord(d->ev0, d->stream));
-    if (n_elig) {
-        const uint32_t path_cap = (uint32_t)std::min<uint64_t>((uint64_t)n * (2 * TILE_MAP_CAP + TILE_EDIT_CAP), 0xfffffff0ull);
-        if ((rc = d_elig.upload(elig.data(), n, d->stream)) || (rc = d_tileoff.upload(toff.data(), n, d->stream)) || (rc = d_tiles.reserve(units * 16 + 16)) ||
-            (rc = d_lists.reserve(TILE_CLASSES * (size_t)n)) || (rc = d_tc.reserve(1)) || (rc = d_res.reserve(n)) || (rc = d_paths.reserve(path_cap))) return rc;
-        GB_CUDA(cudaMemsetAsync(d_tc.ptr, 0, sizeof(TileCounters), d->stream));
-        GB_CUDA(cudaMemsetAsync(d_res.ptr, 0xff, sizeof(TileResult) * (size_t)n, d->stream));
-        PackBatch pk;
-        pk.tree_parent = d_par.ptr; pk.tree_node = d_node.ptr; pk.tree_off = d_toff.ptr; pk.root_trim = d_trim.ptr;
-        pk.query = d_q.ptr; pk.query_off = d_qoff.ptr; pk.max_gap = d_gap.ptr; pk.n = n; pk.tiles = d_tiles.ptr; pk.tile_off = d_tileoff.ptr;
-        for (int c = 0; c < TILE_CLASSES; c++) pk.lists[c] = d_lists.ptr + (size_t)c * n;
-        pk.list_count = d_tc.ptr->list_count; pk.eligible = d_elig.ptr;
-        pack_tiles_kernel<<<(n + 7) / 8, 256, 0, d->stream>>>(d->ix, d->sc, pk);
+        int rc;
+        if ((rc = query_columns(max_q, Lc))) return rc;
+        GB_CUDA(cudaSetDevice(d->device));
+        DevBuf<int32_t> d_par; DevBuf<uint32_t> d_node, d_trim, d_gap, d_counter; DevBuf<uint64_t> d_toff, d_qoff;
+        DevBuf<uint8_t> d_q, d_ws; SeamOutBufs out;
+        const uint64_t nt = tree_off[n], nq = query_off[n];
+        if ((rc = d_par.upload(tree_parent, nt ? nt : 1, d->stream, nt))) return rc;
+        if ((rc = d_node.upload(tree_node, nt ? nt : 1, d->stream, nt))) return rc;
+        if ((rc = d_toff.upload(tree_off, n + 1, d->stream))) return rc;
+        if ((rc = d_trim.upload(root_trim, n, d->stream))) return rc;
+        if ((rc = d_gap.upload(max_gap, n, d->stream))) return rc;
+        if ((rc = d_q.upload(query, nq ? nq : 1, d->stream, nq))) return rc;
+        if ((rc = d_qoff.upload(query_off, n + 1, d->stream))) return rc;
+        if ((rc = out.reserve(n, map_cap, edit_cap))) return rc;
+        if ((rc = d_counter.reserve(4))) return rc;
+        GB_CUDA(cudaMemsetAsync(d_counter.ptr, 0, 16, d->stream));
+        const size_t smem = dp_smem_per_warp(Lc) * XP_WARPS;
+        if (smem > 48 * 1024) GB_CUDA(cudaFuncSetAttribute(xdrop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        uint32_t grid = std::min<uint32_t>((uint32_t)d->n_sms * 2, (n + XP_WARPS - 1) / XP_WARPS);
+        const uint32_t tb_cells = 2 * 1024 * 1024;
+        const size_t ws_stride = tail_ws_bytes(Lc, tb_cells);
+        if ((rc = d_ws.reserve(ws_stride * grid * XP_WARPS))) return rc;
+        XdropBatch b;
+        b.tree_parent = d_par.ptr; b.tree_node = d_node.ptr; b.tree_off = d_toff.ptr; b.root_trim = d_trim.ptr;
+        b.query = d_q.ptr; b.query_off = d_qoff.ptr; b.max_gap = d_gap.ptr; b.n = n; b.Lc = Lc; b.out = out.view;
+        b.ws_base = d_ws.ptr; b.ws_stride = ws_stride; b.tb_cells = tb_cells;
+        b.work_counter = d_counter.ptr;
+        // ---- problems the int16 tile kernel can hold run there (the production path of the tails); the rest on the int32 sweep ----
+        std::vector<uint8_t> elig(n, 0); std::vector<uint32_t> toff(n, 0);
+        uint64_t units = 0; uint32_t n_elig = 0;
+        if (d->use_tiles) {
+            for (uint32_t i = 0; i < n; i++) {
+                const uint32_t ntree = (uint32_t)(tree_off[i + 1] - tree_off[i]), m = (uint32_t)(query_off[i + 1] - query_off[i]);
+                const uint32_t bases = (uint32_t)std::min<uint64_t>(prob_bases[i], 0xffffffffu);
+                if (!tile_eligible(d->sc, m, std::max(max_gap[i], 1u), ntree, bases, prob_depth[i])) continue;
+                elig[i] = 1; toff[i] = (uint32_t)units; units += tile_bytes(ntree, bases, m) / 16; n_elig++;
+            }
+        }
+        DevBuf<uint8_t> d_elig, d_tiles; DevBuf<uint32_t> d_tileoff, d_lists, d_paths; DevBuf<TileCounters> d_tc; DevBuf<TileResult> d_res;
+        GB_CUDA(cudaEventRecord(d->ev0, d->stream));
+        if (n_elig) {
+            const uint32_t path_cap = (uint32_t)std::min<uint64_t>((uint64_t)n * (2 * TILE_MAP_CAP + TILE_EDIT_CAP), 0xfffffff0ull);
+            if ((rc = d_elig.upload(elig.data(), n, d->stream)) || (rc = d_tileoff.upload(toff.data(), n, d->stream)) || (rc = d_tiles.reserve(units * 16 + 16)) ||
+                (rc = d_lists.reserve(TILE_CLASSES * (size_t)n)) || (rc = d_tc.reserve(1)) || (rc = d_res.reserve(n)) || (rc = d_paths.reserve(path_cap))) return rc;
+            GB_CUDA(cudaMemsetAsync(d_tc.ptr, 0, sizeof(TileCounters), d->stream));
+            GB_CUDA(cudaMemsetAsync(d_res.ptr, 0xff, sizeof(TileResult) * (size_t)n, d->stream));
+            PackBatch pk;
+            pk.tree_parent = d_par.ptr; pk.tree_node = d_node.ptr; pk.tree_off = d_toff.ptr; pk.root_trim = d_trim.ptr;
+            pk.query = d_q.ptr; pk.query_off = d_qoff.ptr; pk.max_gap = d_gap.ptr; pk.n = n; pk.tiles = d_tiles.ptr; pk.tile_off = d_tileoff.ptr;
+            for (int c = 0; c < TILE_CLASSES; c++) pk.lists[c] = d_lists.ptr + (size_t)c * n;
+            pk.list_count = d_tc.ptr->list_count; pk.eligible = d_elig.ptr;
+            pack_tiles_kernel<<<(n + 7) / 8, 256, 0, d->stream>>>(d->ix, d->sc, pk);
+            d->launches++;
+            GB_CUDA(cudaGetLastError());
+            d->kt_reset();
+            if ((rc = launch_tile_kernels(d, d_tiles.ptr, d_tileoff.ptr, d_lists.ptr, n, d_tc.ptr->list_count, d_tc.ptr->work, d_res.ptr, d_paths.ptr,
+                                          path_cap, &d_tc.ptr->path_words))) return rc;
+            b.skip = d_elig.ptr;
+            unpack_tile_results_kernel<<<(n + 7) / 8, 256, 0, d->stream>>>(b, d_res.ptr, d_paths.ptr);
+            d->launches++;
+            GB_CUDA(cudaGetLastError());
+        } else b.skip = nullptr;
+        // the int32 sweep takes the problems not eligible for a tile and those whose tile ended FULL; the latter are known only
+        // on the device, so it runs after the tiles too and skips the problems they finished
+        xdrop_kernel<<<grid, XP_WARPS * 32, smem, d->stream>>>(d->ix, d->sc, b);
         d->launches++;
         GB_CUDA(cudaGetLastError());
-        d->kt_reset();
-        if ((rc = launch_tile_kernels(d, d_tiles.ptr, d_tileoff.ptr, d_lists.ptr, n, d_tc.ptr->list_count, d_tc.ptr->work, d_res.ptr, d_paths.ptr,
-                                      path_cap, &d_tc.ptr->path_words))) return rc;
-        b.skip = d_elig.ptr;
-        unpack_tile_results_kernel<<<(n + 7) / 8, 256, 0, d->stream>>>(b, d_res.ptr, d_paths.ptr);
-        d->launches++;
-        GB_CUDA(cudaGetLastError());
-    } else b.skip = nullptr;
-    // the int32 sweep takes the problems not eligible for a tile and those whose tile ended FULL; the latter are known only
-    // on the device, so it runs after the tiles too and skips the problems they finished
-    xdrop_kernel<<<grid, XP_WARPS * 32, smem, d->stream>>>(d->ix, d->sc, b);
-    d->launches++;
-    GB_CUDA(cudaGetLastError());
-    d->last_tile_problems = n_elig;
-    GB_CUDA(cudaEventRecord(d->ev1, d->stream));
-    return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+        d->last_tile_problems = n_elig;
+        GB_CUDA(cudaEventRecord(d->ev1, d->stream));
+        return out.download(d, n, score, maps, edits, n_maps, n_edits, status);
+    });
 }

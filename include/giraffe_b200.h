@@ -437,6 +437,35 @@ int gb_map_paired_job(gb_device* dev, const gb_map_params* p, gb_fragment_distri
                       gb_alignment* aln, gb_mapping* mappings, uint64_t mapping_pool_cap, uint32_t* edits, uint64_t edit_pool_cap,
                       uint8_t* status, uint8_t* pair_route, uint64_t* n_mappings_used, uint64_t* n_edits_used);
 
+/* gb_map_paired_job for reads already in HBM: d_reads, d_quals (may be NULL), d_read_off, d_aln, d_mappings, d_edits,
+ * d_status and d_pair_route (may be NULL) are DEVICE addresses; p, f and the two counts are on the host.  For the same reads,
+ * parameters and distribution state the outputs are exactly gb_map_paired_job's: every record field, the pools up to the
+ * used counts in the same order (training pairs in input order, then the remaining pairs, then the buffered pairs in
+ * buffer order), status, routes and the state of f afterwards.  d_read_off may start at any value and may leave gaps
+ * between reads; every read is at most max_read_len <= 512 long (a longer one is GB_ERR_ARG).  Refused with GB_ERR_ARG
+ * before any work: a NULL p or f, a NULL required array when n_reads > 0, an odd n_reads, max_multimaps != 1,
+ * max_read_len > 512.  n_reads == 0 returns GB_OK and leaves f as it is.  GB_ERR_CAPACITY when a pool is too small: every
+ * sub-batch is sized before it is copied, so nothing is written past mapping_pool_cap / edit_pool_cap.  One call is one
+ * input: when the pairs run out before the sample fills, f is finalized with what it has (the 0 +- 1 it starts with when
+ * nothing was registered, whose pairs then take map_paired's single-end fallback), so a streaming caller's later calls map
+ * fully paired; the ambiguous buffer does not outlive the call.
+ * The call is synchronous (it runs on the handle's stream and returns with the records in place): each training window
+ * (training_window pairs, 0 selects 2048, at most half the map chunk) is mapped single-ended, classified on the device and
+ * copied back once (the cut and the lengths to register); the remaining and the buffered pairs are gathered into
+ * zero-based sub-batches of at most the map chunk (GIRAFFE_B200_MAP_CHUNK, 2^20 reads) and mapped paired.  A sub-batch
+ * that overflows the intermediate pools is redone with them doubled, as in gb_map_batch.  Workspace on the handle (kept,
+ * grown on demand), per read of the largest sub-batch: 8 * mapping_cap_per_read + 4 * edit_cap_per_read + 57 bytes (1.5 KB
+ * with the default caps) plus 2 * max_read_len for the gathered reads and qualities; 4 bytes per pair of the call for the
+ * buffer; 28 bytes per pair of a training window. */
+int gb_map_paired_job_device(gb_device* dev, const gb_map_params* p, gb_fragment_distribution* f, uint32_t training_window,
+                             uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals, const uint64_t* d_read_off,
+                             uint32_t max_read_len,
+                             gb_alignment* d_aln, gb_mapping* d_mappings, uint64_t mapping_pool_cap,
+                             uint32_t* d_edits, uint64_t edit_pool_cap, uint8_t* d_status, uint8_t* d_pair_route,
+                             uint64_t* n_mappings_used, uint64_t* n_edits_used);
+/* The training windows of the last gb_map_paired_job_device call on this handle and the host-clocked time they took (ms). */
+int gb_paired_job_stats(const gb_device* dev, uint32_t* training_windows, double* training_ms);
+
 /* ---- emission (host side, no device work) ---------------------------------------------------
  * giraffe_main.cpp:2209-2226 hands alignments to a vg::io::AlignmentEmitter (libvgio @ d029989,
  * absent from the reference tree).  These two write the same information as text, one line per
@@ -571,7 +600,8 @@ int gb_fastq_parse_device(gb_device* dev, uint32_t n_inputs, const uint8_t* cons
 /* Device-pointer variant of both (paired != 0 selects map_paired): every pointer is a DEVICE
  * address (inputs already resident in HBM, outputs stay in HBM); all reads are at most
  * max_read_len long; d_aln holds n_reads * p->max_multimaps records (rank-major, as gb_map_batch);
- * d_totals[2] (device) receives {mappings used, edits used}.  The call only
+ * d_totals[2] (device) receives {mappings used, edits used}.  With paired != 0, d_read_off[0] must be 0 and
+ * d_read_off[n_reads] <= n_reads * max_read_len (the paired working copy of the reads is addressed by them).  The call only
  * enqueues work on the handle's stream (gb_device_set_stream) and returns; use
  * gb_device_synchronize or stream ordering before reading the outputs. */
 int gb_map_batch_device(gb_device* dev, const gb_map_params* p, int paired, uint32_t n_reads,

@@ -177,6 +177,8 @@ def load_library() -> C.CDLL:
         "gb_fragment_is_finalized": (st, [vp]),
         "gb_fragment_sample_size": (u64, [vp]),
         "gb_map_paired_job": (st, [vp, C.POINTER(MapParams), vp, u32, u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, vp, vp, vp]),
+        "gb_map_paired_job_device": (st, [vp, C.POINTER(MapParams), vp, u32, u32, vp, vp, vp, u32, vp, vp, u64, vp, u64, vp, vp, vp, vp]),
+        "gb_paired_job_stats": (st, [vp, C.POINTER(u32), C.POINTER(C.c_double)]),
         "gb_emit_gaf": (st, [fix, *emit]),
         "gb_emit_json": (st, [fix, *emit]),
         "gb_emit_gam": (st, [fix, *emit]),
@@ -757,6 +759,24 @@ class Device:
                                      C.byref(used[0]), C.byref(used[1])), "gb_map_paired_job")
         self.last_used = (used[0].value, used[1].value)
         return aln, maps, edits, status, route
+
+    def map_paired_job_device(self, distribution, n_reads, reads, quals, read_off, max_read_len, aln, maps, map_cap, edits, edit_cap,
+                              status, route=None, params=None, training_window=0):
+        """gb_map_paired_job_device on device pointers (ints, or None for quals / route), in the style of the raw
+        gb_map_batch_device calls: reads / quals / read_off are the inputs, aln / maps / edits / status / route receive the
+        records.  Synchronous.  Returns (rc, mappings used, edits used) without raising, so callers can test refusals."""
+        lib = load_library()
+        p = params or default_map_params()
+        used = (C.c_uint64(), C.c_uint64())
+        rc = lib.gb_map_paired_job_device(self._h, C.byref(p), distribution._h, training_window, n_reads, reads, quals, read_off, max_read_len,
+                                          aln, maps, map_cap, edits, edit_cap, status, route, C.byref(used[0]), C.byref(used[1]))
+        return rc, used[0].value, used[1].value
+
+    def paired_job_stats(self):
+        """(training windows, host-clocked training ms) of the last gb_map_paired_job_device call."""
+        n, ms = C.c_uint32(), C.c_double()
+        _check(load_library().gb_paired_job_stats(self._h, C.byref(n), C.byref(ms)), "gb_paired_job_stats")
+        return n.value, ms.value
 
     def seed_stage(self, rbuf, qbuf, read_off, params=None, paired=False, per_read=(160, 1024, 64, 64, 1024)):
         """gb_debug_seed_stage: (reads, minimizers, seeds, clusters, items, item_seeds) as structured arrays."""

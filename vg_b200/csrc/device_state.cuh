@@ -109,6 +109,23 @@ static_assert(offsetof(MapCursors, tile_path_words) == offsetof(MapCursors, tile
 
 } // namespace gb
 
+struct gb_device;
+namespace gb {
+
+// map.cu: one batch of reads already in HBM through every stage, records compacted into out_maps / out_edits (paired:
+// d_read_off[0] == 0 and d_read_off[n_reads] <= total_bases, the size of the working copy of the reads).
+int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
+               const uint64_t* d_read_off, uint32_t max_len, uint64_t total_bases,
+               gb_alignment* d_aln, uint8_t* d_status, bool paired,
+               gb_mapping* out_maps, uint64_t out_map_cap, uint32_t* out_edits, uint64_t out_edit_cap,
+               const uint64_t* d_run_base, uint32_t read_base, uint64_t* d_totals, uint32_t* d_overflow);
+
+// A batch that set MapCursors::pool_overflow is redone with the intermediate pools doubled: this doubles them, or
+// refuses (GB_ERR_CAPACITY) once they are at 1024x the per-read averages.
+int grow_pools_for_rerun(gb_device* d);
+
+} // namespace gb
+
 struct gb_device {
     int device = 0;
     int n_sms = 0;
@@ -199,4 +216,14 @@ struct gb_device {
     gb::DevBuf<uint8_t> bgzf_ws;           // gb_bgzf_compress_device: member slots, token slots, member sizes and offsets
     gb::DevBuf<uint8_t> inflate_ws;        // gb_bgzf_decompress_device: the member list and the walk's summary
     gb::DevBuf<uint8_t> fastq_ws;          // gb_fastq_parse_device: line ends, per-read lengths and offsets, scan temporaries
+    // gb_map_paired_job_device: one sub-batch's records, its gathered reads, the per-pair training arrays, the buffered pairs
+    struct PairedJobWs {
+        gb::DevBuf<gb_alignment> aln;
+        gb::DevBuf<uint8_t> status, reads, quals, scan_tmp;
+        gb::DevBuf<gb_mapping> maps;
+        gb::DevBuf<uint32_t> edits, pair, buffered;
+        gb::DevBuf<uint64_t> off, totals, append_off;
+        gb::DevBuf<int64_t> out;
+    } pj;
+    uint32_t pj_windows = 0; double pj_training_ms = 0.0;      // training windows of the last such call and their host-clocked time
 };

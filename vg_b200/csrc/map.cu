@@ -549,6 +549,12 @@ int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const ui
     return GB_OK;
 }
 
+int grow_pools_for_rerun(gb_device* d) {
+    if (d->pool_scale >= 1024.0) { g_last_error = "intermediate pools overflow even at 1024x the per-read averages; use a smaller GIRAFFE_B200_MAP_CHUNK"; return GB_ERR_CAPACITY; }
+    d->pool_scale *= 2.0; d->pool_reruns++;
+    return GB_OK;
+}
+
 } // namespace gb
 
 // Host-buffer entry: chunks of <= map_chunk reads are copied in, mapped, compacted and copied out,
@@ -673,8 +679,7 @@ static int map_batch_host(gb_device* d, const gb_map_params* hp, bool paired,
             rc = finish(finished);
             if (rc == RERUN) {
                 drain();
-                if (d->pool_scale >= 1024.0) { g_last_error = "intermediate pools overflow even at 1024x the per-read averages; use a smaller GIRAFFE_B200_MAP_CHUNK"; return GB_ERR_CAPACITY; }
-                d->pool_scale *= 2.0; d->pool_reruns++;
+                if ((rc = gb::grow_pools_for_rerun(d))) return rc;
                 const uint64_t run[2] = {map_used, edit_used};
                 GB_CUDA(cudaMemcpy(d->c_run.ptr, run, sizeof run, cudaMemcpyHostToDevice));
                 used[0] = used[1] = false;

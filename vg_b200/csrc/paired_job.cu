@@ -8,12 +8,12 @@
 // bookkeeping the reference also runs single-threaded (giraffe_main.cpp:2253), one window of pairs at a time.
 #include "giraffe_b200.h"
 #include "device_state.cuh"
+#include "fragment_distribution.h"
 
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <limits>
-#include <set>
 #include <vector>
 
 using gb::g_last_error;
@@ -45,33 +45,18 @@ double phi_inv(double p) {
 
 } // namespace
 
-struct gb_fragment_distribution {
-    std::multiset<double> lengths;
-    bool is_fixed = false;
-    double robust_estimation_fraction = 0.95;
-    uint64_t maximum_sample_size = 1000, reestimation_frequency = 1000;
-    double mu = 0.0, sigma = 1.0;
-
-    void estimate() {
-        // trimmed sample, then the method of moments for a normal truncated at +-a
-        const size_t to_skip = (size_t)(lengths.size() * (1.0 - robust_estimation_fraction) * 0.5);
-        auto begin = lengths.begin(); auto end = lengths.end();
-        for (size_t i = 0; i < to_skip; i++) { ++begin; --end; }
-        double count = 0.0, sum = 0.0, sum_of_sqs = 0.0;
-        for (auto it = begin; it != end; ++it) { count += 1.0; sum += *it; sum_of_sqs += (*it) * (*it); }
-        mu = sum / count;
-        const double raw_var = sum_of_sqs / count - mu * mu;
-        const double a = phi_inv(1.0 - 0.5 * (1.0 - robust_estimation_fraction));
-        const double pdf_a = 0.3989422804014327 * std::exp(-0.5 * a * a);
-        sigma = std::sqrt(raw_var / (1.0 - 2.0 * a * pdf_a));
-    }
-    void add(int64_t length) {
-        if (is_fixed) return;
-        lengths.insert((double)length);
-        if (lengths.size() == maximum_sample_size) { estimate(); is_fixed = true; }
-        else if (lengths.size() % reestimation_frequency == 0) estimate();
-    }
-};
+void gb_fragment_distribution::estimate() {
+    const size_t to_skip = (size_t)(lengths.size() * (1.0 - robust_estimation_fraction) * 0.5);
+    auto begin = lengths.begin(); auto end = lengths.end();
+    for (size_t i = 0; i < to_skip; i++) { ++begin; --end; }
+    double count = 0.0, sum = 0.0, sum_of_sqs = 0.0;
+    for (auto it = begin; it != end; ++it) { count += 1.0; sum += *it; sum_of_sqs += (*it) * (*it); }
+    mu = sum / count;
+    const double raw_var = sum_of_sqs / count - mu * mu;
+    const double a = phi_inv(1.0 - 0.5 * (1.0 - robust_estimation_fraction));
+    const double pdf_a = 0.3989422804014327 * std::exp(-0.5 * a * a);
+    sigma = std::sqrt(raw_var / (1.0 - 2.0 * a * pdf_a));
+}
 
 extern "C" gb_fragment_distribution* gb_fragment_create(uint64_t maximum_sample_size, uint64_t reestimation_frequency, double robust_estimation_fraction) {
     if (!(robust_estimation_fraction > 0.0 && robust_estimation_fraction < 1.0) || reestimation_frequency == 0) {

@@ -121,12 +121,7 @@ __device__ inline bool fast_pair(const DevIndex& ix, const MapParamsDev& P, cons
             if (n_ext > 0 && ext_full(ext[0]) && ext[0].mismatches <= 4) set_score[s] = ext[0].score;
             else set_score[s] = score_extension_group(ext, n_ext, L[r], sc.gap_open, sc.gap_extend);
         }
-        for (uint32_t s = 0; s < S; s++) { uint32_t j = s; while (j > 0 && set_score[s] > set_score[set_order[j - 1]]) { set_order[j] = set_order[j - 1]; j--; } set_order[j] = (uint8_t)s; }
-        {
-            uint32_t ties = 0;
-            while (ties < S && !(set_score[set_order[0]] > set_score[set_order[ties]])) ties++;
-            for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = set_order[j]; set_order[j] = set_order[i]; set_order[i] = t; }
-        }
+        sort_shuffling_ties(S, [&](uint32_t x, uint32_t y) { return set_score[x] > set_score[y]; }, set_order, rng);
         const double set_cutoff = S == 0 ? 0.0 : (double)set_score[set_order[0]] - P.extension_set_score_threshold;
         uint32_t unskipped = 0;
         for (uint32_t oi = 0; oi < S; oi++) {
@@ -173,46 +168,25 @@ __device__ inline bool fast_pair(const DevIndex& ix, const MapParamsDev& P, cons
         return true;
     };
     double pair_score[FAST_MAX_PAIRS]; int64_t pair_dist[FAST_MAX_PAIRS]; uint8_t pair_c0[FAST_MAX_PAIRS], pair_c1[FAST_MAX_PAIRS], pair_better[FAST_MAX_PAIRS];
-    uint32_t n_pairs = 0; bool found_pair = false;
-    uint8_t unpaired[FAST_MAX_CANDS]; uint32_t n_unpaired = 0;
-    const uint32_t n_frag_slots = ps.n_fragments + 1;
-    for (uint32_t f = 0; f < n_frag_slots; f++) {
-        bool has0 = false, has1 = false;
-        for (uint32_t c = 0; c < n_cand; c++) if (cand[c].frag == f) { if (cand[c].read == 0) has0 = true; else has1 = true; }
-        if (has0 && has1) {
-            found_pair = true;
-            for (uint32_t c0 = 0; c0 < n_cand; c0++) {
-                if (cand[c0].frag != f || cand[c0].read != 0) continue;
-                for (uint32_t c1 = 0; c1 < n_cand; c1++) {
-                    if (cand[c1].frag != f || cand[c1].read != 1) continue;
-                    if (n_pairs >= FAST_MAX_PAIRS) return false;
-                    uint32_t fn, fo, ln, le, x0, x1, x2, x3;
-                    extension_ends(ix, ext_of(cand[c0]), ev_path(a.ev, cand[c0].item), fn, fo, x0, x1);
-                    extension_ends(ix, ext_of(cand[c1]), ev_path(a.ev, cand[c1].item), x2, x3, ln, le);
-                    const int64_t dist = oriented_distance(ix, fn, fo, ln, le);
-                    const double dev = (double)dist - a.frag_mean;
-                    const double ll = (-dev * dev / (2.0 * a.frag_sd * a.frag_sd)) / P.log_base;
-                    const double sc_sum = (double)cand[c0].score + (double)cand[c1].score + ll;
-                    const double worse = fmin((double)cand[c0].score, (double)cand[c1].score);
-                    pair_score[n_pairs] = fmax(sc_sum, worse); pair_dist[n_pairs] = dist;
-                    pair_c0[n_pairs] = (uint8_t)c0; pair_c1[n_pairs] = (uint8_t)c1; pair_better[n_pairs] = ps.better_cluster_count[f];
-                    n_pairs++;
-                }
-            }
-        } else {
-            for (uint32_t r = 0; r < 2; r++) for (uint32_t c = 0; c < n_cand; c++) if (cand[c].frag == f && cand[c].read == r) unpaired[n_unpaired++] = (uint8_t)c;
-        }
-    }
+    uint32_t n_pairs, n_unpaired; bool found_pair;
+    uint8_t unpaired[FAST_MAX_CANDS];
+    auto frag_of = [&](uint32_t c) { return (uint32_t)cand[c].frag; };
+    auto read_of = [&](uint32_t c) { return (uint32_t)cand[c].read; };
+    auto score_of = [&](uint32_t c) { return cand[c].score; };
+    auto dist_of = [&](uint32_t c0, uint32_t c1) {
+        uint32_t fn, fo, ln, le, x0, x1, x2, x3;
+        extension_ends(ix, ext_of(cand[c0]), ev_path(a.ev, cand[c0].item), fn, fo, x0, x1);
+        extension_ends(ix, ext_of(cand[c1]), ev_path(a.ev, cand[c1].item), x2, x3, ln, le);
+        return oriented_distance(ix, fn, fo, ln, le);
+    };
+    if (!collect_pairs<FAST_MAX_PAIRS>(n_cand, ps.n_fragments + 1, frag_of, read_of, score_of, dist_of, ps.better_cluster_count, a.frag_mean, a.frag_sd,
+                                       P.log_base, pair_score, pair_dist, pair_c0, pair_c1, pair_better, n_pairs, found_pair, unpaired, n_unpaired))
+        return false;
     bool done = false;
     if (n_unpaired > 0 && P.max_rescue_attempts != 0) return false;     // mate rescue is warp work
     if (n_unpaired > 0 && !found_pair) {
-        int best_c[2] = {-1, -1}; int32_t best_score[2] = {0, 0};
-        for (uint32_t u = 0; u < n_unpaired; u++) {
-            const uint32_t c = unpaired[u]; const uint32_t r = cand[c].read;
-            bool beats = cand[c].score > best_score[r];
-            if (!beats && cand[c].score == best_score[r]) beats = (rng_next(rng) % 2) != 0;
-            if (beats) { best_c[r] = (int)c; best_score[r] = cand[c].score; }
-        }
+        int best_c[2]; int32_t best_score[2];
+        best_unpaired_per_end(unpaired, n_unpaired, read_of, score_of, rng, best_c, best_score);
         for (uint32_t r = 0; r < 2; r++) {
             out[r].mapq = 1;
             if (best_c[r] >= 0 && !write_cand(r, cand[best_c[r]])) return false;
@@ -220,18 +194,12 @@ __device__ inline bool fast_pair(const DevIndex& ix, const MapParamsDev& P, cons
         done = true;
     } else if (n_pairs > 0) {
         uint8_t po[FAST_MAX_PAIRS];
-        for (uint32_t q = 0; q < n_pairs; q++) { uint32_t j = q; while (j > 0 && pair_score[q] > pair_score[po[j - 1]]) { po[j] = po[j - 1]; j--; } po[j] = (uint8_t)q; }
-        {
-            uint32_t ties = 0;
-            while (ties < n_pairs && !(pair_score[po[0]] > pair_score[po[ties]])) ties++;
-            for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = po[j]; po[j] = po[i]; po[i] = t; }
-        }
+        sort_shuffling_ties(n_pairs, [&](uint32_t x, uint32_t y) { return pair_score[x] > pair_score[y]; }, po, rng);
         double scores_sorted[FAST_MAX_PAIRS];
         for (uint32_t q = 0; q < n_pairs; q++) scores_sorted[q] = pair_score[po[q]];
         const uint32_t wp = po[0];
         const double uncapped_mapq = scores_sorted[0] == 0 ? 0.0 : max_mapping_quality(scores_sorted, n_pairs, P.log_base);
-        double fragment_cluster_cap = INFINITY;
-        if (pair_better[wp] > 1) fragment_cluster_cap = -10.0 * log10(1.0 - (1.0 / (double)pair_better[wp]));
+        const double cluster_cap = fragment_cluster_cap(pair_better[wp]);
         double caps[2];
         for (uint32_t r = 0; r < 2; r++) {
             // explored-minimizer count bound for the per-thread tables
@@ -244,15 +212,8 @@ __device__ inline bool fast_pair(const DevIndex& ix, const MapParamsDev& P, cons
         }
         const uint32_t cwin[2] = {pair_c0[wp], pair_c1[wp]};
         for (uint32_t r = 0; r < 2; r++) {
-            const double escape_bonus = uncapped_mapq < 2147483647.0 ? 1.0 : 2.0;
-            const double mapq_cap = fmin(fragment_cluster_cap, (caps[0] + caps[1]) * escape_bonus);
-            double capped = fmin(mapq_cap, uncapped_mapq);
-            if (pair_dist[wp] == INT64_MAX) capped = capped / 2.0;
-            double read_mapq = fmax(fmin(capped, 120.0) / 2.0, 0.0);
             if (!write_cand(r, cand[cwin[r]])) return false;
-            if (out[r].n_mappings == 0) read_mapq = 0;
-            out[r].mapq = (uint8_t)(int32_t)read_mapq;
-            out[r].mapq_uncapped = (float)uncapped_mapq; out[r].mapq_explored_cap = (float)mapq_cap;
+            pair_read_mapq(uncapped_mapq, cluster_cap, caps[0] + caps[1], pair_dist[wp] == INT64_MAX, INFINITY, out[r]);
         }
         done = true;
     } else {
@@ -290,12 +251,7 @@ __device__ inline bool fast_read(const DevIndex& ix, const MapParamsDev& P, cons
         if (n_ext > 0 && ext_full(ext[0]) && ext[0].mismatches <= 4) set_score[s] = ext[0].score;
         else set_score[s] = score_extension_group(ext, n_ext, L, sc.gap_open, sc.gap_extend);
     }
-    for (uint32_t s = 0; s < S; s++) { uint32_t j = s; while (j > 0 && set_score[s] > set_score[set_order[j - 1]]) { set_order[j] = set_order[j - 1]; j--; } set_order[j] = (uint8_t)s; }
-    {
-        uint32_t ties = 0;
-        while (ties < S && !(set_score[set_order[0]] > set_score[set_order[ties]])) ties++;
-        for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = set_order[j]; set_order[j] = set_order[i]; set_order[i] = t; }
-    }
+    sort_shuffling_ties(S, [&](uint32_t x, uint32_t y) { return set_score[x] > set_score[y]; }, set_order, rng);
     const double set_cutoff = S == 0 ? 0.0 : (double)set_score[set_order[0]] - P.extension_set_score_threshold;
     uint32_t unskipped = 0;
     for (uint32_t oi = 0; oi < S; oi++) {
@@ -327,28 +283,21 @@ __device__ inline bool fast_read(const DevIndex& ix, const MapParamsDev& P, cons
     if (n_cand == 0) { scores_sorted[0] = 0.0; n_scores = 1; }
     else {
         uint8_t co[FAST_MAX_CANDS];
-        for (uint32_t c = 0; c < n_cand; c++) { uint32_t j = c; while (j > 0 && cand[c].score > cand[co[j - 1]].score) { co[j] = co[j - 1]; j--; } co[j] = (uint8_t)c; }
-        uint32_t ties = 0;
-        while (ties < n_cand && !(cand[co[0]].score > cand[co[ties]].score)) ties++;
-        for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = co[j]; co[j] = co[i]; co[i] = t; }
+        sort_shuffling_ties(n_cand, [&](uint32_t x, uint32_t y) { return cand[x].score > cand[y].score; }, co, rng);
         for (uint32_t c = 0; c < n_cand; c++) scores_sorted[c] = (double)cand[co[c]].score;
         n_scores = n_cand; win = co[0];
     }
-    double mapq = win >= 0 ? max_mapping_quality(scores_sorted, n_scores, P.log_base) : 0.0;
-    const double escape_bonus = mapq < 2147483647.0 ? 1.0 : 2.0;
+    const double mapq = win >= 0 ? max_mapping_quality(scores_sorted, n_scores, P.log_base) : 0.0;
     uint32_t n_exp = 0;
 #pragma unroll
     for (uint32_t x = 0; x < PRESENT_WORDS; x++) n_exp += __popc(explored[x]);
     if (n_exp > FAST_MAX_EXPLORED) return false;
     uint64_t mp[FAST_MAX_EXPLORED]; double cbuf[FAST_MAX_EXPLORED + 1];
-    const double cap = escape_bonus * faster_cap(P, a.minimizers + rs.min_off, ix.k, explored, rs.min_cnt, qual, L, mp, cbuf);
-    const double mapq_uncapped = mapq;
-    mapq = round(fmin(cap, fmin(mapq, 60.0)));
-    mapq = fmax(fmin(mapq, 60.0), 0.0);
+    const double cap = faster_cap(P, a.minimizers + rs.min_off, ix.k, explored, rs.min_cnt, qual, L, mp, cbuf);
     gb_alignment out;
-    out.read_id = r; out.score = 0; out.mapq = (uint8_t)mapq; out.flags = 0; out.n_mappings = 0; out.n_edits = 0;
+    out.read_id = r; out.score = 0; out.flags = 0; out.n_mappings = 0; out.n_edits = 0;
     out.mapping_off = r * P.mapping_cap; out.edit_off = r * P.edit_cap;
-    out.mapq_uncapped = (float)mapq_uncapped; out.mapq_explored_cap = (float)cap;
+    single_end_mapq(mapq, cap, out);
     if (win >= 0) {
         const FastCand& c = cand[win];
         uint32_t nm = 0, ne = 0;

@@ -254,21 +254,125 @@ __device__ inline double faster_cap_warp(const MapParamsDev& P, const DevMinimiz
     return result;
 }
 
-// MappingQualityCalculator::compute_max_mapping_quality (exact, no multiplicities),
-// mapping_quality_calculator.cpp:26-67, :355-364.  Returns the int32-truncated value as double.
-__device__ inline double max_mapping_quality(const double* scores, uint32_t n, double log_base) {
+// MappingQualityCalculator::compute_max_mapping_quality (exact), mapping_quality_calculator.cpp:26-67, :355-364, with
+// the multiplicities of the scores when `mult` is given.  Returns the int32-truncated value as double.
+__device__ inline double max_mapping_quality(const double* scores, uint32_t n, double log_base, const double* mult = nullptr) {
     const double quality_scale_factor = 10.0 / log(10.0);
     double log_sum_exp = -DBL_MAX, to_score = -DBL_MAX;
 #pragma unroll 1
     for (int64_t i = (int64_t)n - 1; i >= 0; --i) {
-        const double score = log_base * scores[i];
+        double score = log_base * scores[i];
         if (score >= to_score) to_score = score;
+        if (mult && mult[i] > 1.0) score += log(mult[i]);
         log_sum_exp = d_add_log(log_sum_exp, score);
     }
-    if (n == 1) log_sum_exp = d_add_log(log_sum_exp, 0.0);
+    if (n == 1 && (!mult || mult[0] <= 1.0)) log_sum_exp = d_add_log(log_sum_exp, 0.0);
     const double direct = -quality_scale_factor * d_subtract_log(0.0, to_score - log_sum_exp);
     const double mq = isinf(direct) ? 2147483647.0 : direct;
     return (double)(int32_t)mq;
+}
+
+// Single-end MAPQ (:1146-1188): the explored cap (doubled past the escape threshold) and 60 bound the uncapped MAPQ.
+// Fills the MAPQ fields of the primary record.
+__device__ __forceinline__ void single_end_mapq(double mapq, double explored_cap, gb_alignment& out) {
+    const double escape_bonus = mapq < 2147483647.0 ? 1.0 : 2.0;
+    const double cap = escape_bonus * explored_cap;
+    const double capped = round(fmin(cap, fmin(mapq, 60.0)));
+    out.mapq = (uint8_t)fmax(fmin(capped, 60.0), 0.0);
+    out.mapq_uncapped = (float)mapq; out.mapq_explored_cap = (float)cap;
+}
+
+// distance_between(aln1, aln2) (:3895-3903) of two finished candidate slots: initial_position(p0) -> final_position(p1)
+__device__ __forceinline__ int64_t distance_between(const DevIndex& ix, const PathBuf& p0, const PathBuf& p1) {
+    const gb_mapping first = p0.maps[0];
+    const uint32_t nm1 = slot_nm(p1), ne1 = slot_ne(p1);
+    const gb_mapping last = p1.maps[nm1 - 1];
+    uint32_t used = 0;
+#pragma unroll 1
+    for (uint32_t x = ne1 - last.n_edits; x < ne1; x++) { const uint32_t wd = p1.edits[x]; const uint32_t op = wd & 3u; if (op != GB_EDIT_INS) used += (op == GB_EDIT_SUB) ? 1u : (wd >> 4); }
+    return oriented_distance(ix, first.node, first.offset, last.node, (uint32_t)last.offset + used);
+}
+
+// score_alignment_pair (:6017-6028): both scores plus the fragment-length log-likelihood, never below the worse score
+__device__ __forceinline__ double score_alignment_pair(int32_t s0, int32_t s1, int64_t dist, double frag_mean, double frag_sd, double log_base) {
+    const double dev = (double)dist - frag_mean;
+    const double ll = (-dev * dev / (2.0 * frag_sd * frag_sd)) / log_base;
+    return fmax((double)s0 + (double)s1 + ll, fmin((double)s0, (double)s1));
+}
+
+// The fragment loop of map_paired (:2108-2208).  Candidates c < n have fragment frag(c), read read(c) (0 or 1) and score
+// score(c).  In each fragment f < n_frag that holds both reads, every (read 0, read 1) combination becomes a pair, scored at
+// distance dist(c0, c1); the candidates of the other fragments go to `unpaired`, read 0 first.  Returns false when the
+// pairs do not fit in MAX_PAIRS.
+template <uint32_t MAX_PAIRS, typename Frag, typename Read, typename Score, typename Dist>
+__device__ __forceinline__ bool collect_pairs(uint32_t n, uint32_t n_frag, Frag frag, Read read, Score score, Dist dist,
+                                              const uint8_t* better_cluster_count, double frag_mean, double frag_sd, double log_base,
+                                              double* pair_score, int64_t* pair_dist, uint8_t* pair_c0, uint8_t* pair_c1, uint8_t* pair_better,
+                                              uint32_t& n_pairs, bool& found_pair, uint8_t* unpaired, uint32_t& n_unpaired) {
+    n_pairs = 0; found_pair = false; n_unpaired = 0;
+#pragma unroll 1
+    for (uint32_t f = 0; f < n_frag; f++) {
+        bool has0 = false, has1 = false;
+#pragma unroll 1
+        for (uint32_t c = 0; c < n; c++) if (frag(c) == f) { if (read(c) == 0) has0 = true; else has1 = true; }
+        if (has0 && has1) {
+            found_pair = true;
+#pragma unroll 1
+            for (uint32_t c0 = 0; c0 < n; c0++) {
+                if (frag(c0) != f || read(c0) != 0) continue;
+#pragma unroll 1
+                for (uint32_t c1 = 0; c1 < n; c1++) {
+                    if (frag(c1) != f || read(c1) != 1) continue;
+                    if (n_pairs >= MAX_PAIRS) return false;
+                    const int64_t d = dist(c0, c1);
+                    pair_score[n_pairs] = score_alignment_pair(score(c0), score(c1), d, frag_mean, frag_sd, log_base); pair_dist[n_pairs] = d;
+                    pair_c0[n_pairs] = (uint8_t)c0; pair_c1[n_pairs] = (uint8_t)c1; pair_better[n_pairs] = better_cluster_count[f];
+                    n_pairs++;
+                }
+            }
+        } else {
+#pragma unroll 1
+            for (uint32_t r = 0; r < 2; r++)
+#pragma unroll 1
+                for (uint32_t c = 0; c < n; c++) if (frag(c) == f && read(c) == r) unpaired[n_unpaired++] = (uint8_t)c;
+        }
+    }
+    return true;
+}
+
+// The best unpaired alignment of each end when no fragment holds a pair (:2216-2236): a LazyRNG coin flip decides a tie
+// with the best so far.  best_c[r] = -1 when end r has none.
+template <typename Read, typename Score>
+__device__ __forceinline__ void best_unpaired_per_end(const uint8_t* unpaired, uint32_t n_unpaired, Read read, Score score, DevRng& rng,
+                                                      int (&best_c)[2], int32_t (&best_score)[2]) {
+    best_c[0] = best_c[1] = -1; best_score[0] = best_score[1] = 0;
+#pragma unroll 1
+    for (uint32_t u = 0; u < n_unpaired; u++) {
+        const uint32_t c = unpaired[u], r = read(c);
+        bool beats = score(c) > best_score[r];
+        if (!beats && score(c) == best_score[r]) beats = (rng_next(rng) % 2) != 0;
+        if (beats) { best_c[r] = (int)c; best_score[r] = score(c); }
+    }
+}
+
+// MAPQ cap from the number of fragment clusters at least as good as the winning pair's, its own included (:2692-2697)
+__device__ __forceinline__ double fragment_cluster_cap(uint32_t better_cluster_count) {
+    return better_cluster_count > 1 ? -10.0 * log10(1.0 - (1.0 / (double)better_cluster_count)) : INFINITY;
+}
+
+// MAPQ of one read of the winning pair (:2727-2762): the fragment-cluster cap, the sum of both reads' explored caps
+// (doubled past the escape threshold) and extra_cap (INFINITY: none) bound the pair's uncapped MAPQ, which is halved when
+// the mates cannot reach each other and then split between the reads.  Fills the MAPQ fields of out once its flags are
+// set: a read without GB_ALN_MAPPED gets 0.
+__device__ __forceinline__ void pair_read_mapq(double uncapped, double cluster_cap, double caps_sum, bool unreachable, double extra_cap,
+                                               gb_alignment& out) {
+    const double escape_bonus = uncapped < 2147483647.0 ? 1.0 : 2.0;
+    const double mapq_cap = fmin(fmin(cluster_cap, caps_sum * escape_bonus), extra_cap);
+    double capped = fmin(mapq_cap, uncapped);
+    if (unreachable) capped = capped / 2.0;
+    const double read_mapq = (out.flags & GB_ALN_MAPPED) ? fmax(fmin(capped, 120.0) / 2.0, 0.0) : 0.0;
+    out.mapq = (uint8_t)(int32_t)read_mapq;
+    out.mapq_uncapped = (float)uncapped; out.mapq_explored_cap = (float)mapq_cap;
 }
 
 // Deferred cluster selection of read 2 of a pair (see cluster_phase_pe): the seeding kernel left every cluster of the read
@@ -339,15 +443,7 @@ __device__ inline uint32_t align_sets(const DevIndex& ix, const MapParamsDev& P,
         if (a.ev.ext_status[item] != GB_ITEM_OK) return a.ev.ext_status[item];
         set_score[s] = score_extension_group(ev_ext(a.ev, item), a.ev.ext_count[item], L, sc.gap_open, sc.gap_extend);
     }
-#pragma unroll 1
-    for (uint32_t s = 0; s < S; s++) { uint32_t j = s; while (j > 0 && set_score[s] > set_score[set_order[j - 1]]) { set_order[j] = set_order[j - 1]; j--; } set_order[j] = (uint8_t)s; }
-    {
-        uint32_t ties = 0;
-#pragma unroll 1
-        while (ties < S && !(set_score[set_order[0]] > set_score[set_order[ties]])) ties++;
-#pragma unroll 1
-        for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = set_order[j]; set_order[j] = set_order[i]; set_order[i] = t; }
-    }
+    sort_shuffling_ties(S, [&](uint32_t x, uint32_t y) { return set_score[x] > set_score[y]; }, set_order, rng);
     const double set_cutoff = S == 0 ? 0.0 : (double)set_score[set_order[0]] - P.extension_set_score_threshold;
     const uint32_t min_sets = paired ? 2u : (uint32_t)P.min_extension_sets;
     uint32_t unskipped = 0;
@@ -420,15 +516,7 @@ __device__ inline uint32_t align_sets(const DevIndex& ix, const MapParamsDev& P,
             nl = find_pareto_frontier(lf, nl); nr = find_pareto_frontier(rf, nr);
 
             uint8_t eo[64]; const uint32_t ne_ = min(n_ext, 64u);
-#pragma unroll 1
-            for (uint32_t j = 0; j < ne_; j++) { uint32_t x = j; while (x > 0 && ext[j].score > ext[eo[x - 1]].score) { eo[x] = eo[x - 1]; x--; } eo[x] = (uint8_t)j; }
-            {
-                uint32_t ties = 0;
-#pragma unroll 1
-                while (ties < ne_ && !(ext[eo[0]].score > ext[eo[ties]].score)) ties++;
-#pragma unroll 1
-                for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = eo[j]; eo[j] = eo[i]; eo[i] = t; }
-            }
+            sort_shuffling_ties(ne_, [&](uint32_t x, uint32_t y) { return ext[x].score > ext[y].score; }, eo, rng);
             const double ecut = ne_ == 0 ? 0.0 : (double)ext[eo[0]].score - (double)P.extension_score_threshold;
             uint32_t e_unskipped = 0;
             uint32_t win_slot = 0xffffffffu, sec_slot = 0xffffffffu;
@@ -590,30 +678,19 @@ __device__ inline uint32_t finalize_se(const DevIndex& ix, const MapParamsDev& P
     uint8_t co[MAX_CANDS];
     if (cl.n == 0) { scores_sorted[0] = 0.0; n_scores = 1; }
     else {
-#pragma unroll 1
-        for (uint32_t c = 0; c < cl.n; c++) { uint32_t j = c; while (j > 0 && cl.score[c] > cl.score[co[j - 1]]) { co[j] = co[j - 1]; j--; } co[j] = (uint8_t)c; }
-        uint32_t ties = 0;
-#pragma unroll 1
-        while (ties < cl.n && !(cl.score[co[0]] > cl.score[co[ties]])) ties++;
-#pragma unroll 1
-        for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = co[j]; co[j] = co[i]; co[i] = t; }
+        sort_shuffling_ties(cl.n, [&](uint32_t x, uint32_t y) { return cl.score[x] > cl.score[y]; }, co, rng);
 #pragma unroll 1
         for (uint32_t c = 0; c < cl.n; c++) scores_sorted[c] = (double)cl.score[co[c]];
         n_scores = cl.n; win = co[0];
     }
     double mapq = 0.0;
     if (win != 0xffffffffu) mapq = max_mapping_quality(scores_sorted, n_scores, P.log_base);
-    const double escape_bonus = mapq < 2147483647.0 ? 1.0 : 2.0;
     double* cbuf = reinterpret_cast<double*>(dps.Hp);       // DP columns are free here (Hp|Ep and Hc|Ec)
     uint64_t* ordbuf = reinterpret_cast<uint64_t*>(dps.Hc);
-    double cap = 0.0;
-    cap = escape_bonus * faster_cap_warp(P, a.minimizers + rs.min_off, ix.k, explored, rs.min_cnt, qual, L, ordbuf, cbuf);
-    const double mapq_uncapped = mapq;
-    mapq = round(fmin(cap, fmin(mapq, 60.0)));
-    mapq = fmax(fmin(mapq, 60.0), 0.0);
+    const double cap = faster_cap_warp(P, a.minimizers + rs.min_off, ix.k, explored, rs.min_cnt, qual, L, ordbuf, cbuf);
 
-    out.read_id = read_idx; out.score = 0; out.mapq = (uint8_t)mapq; out.flags = 0; out.n_mappings = 0; out.n_edits = 0;
-    out.mapq_uncapped = (float)mapq_uncapped; out.mapq_explored_cap = (float)cap;
+    out.read_id = read_idx; out.score = 0; out.flags = 0; out.n_mappings = 0; out.n_edits = 0;
+    single_end_mapq(mapq, cap, out);
     if (win != 0xffffffffu) {
         PathBuf pb = slot_buf(cand_base, cl.slot[win], map_cap, edit_cap);
         const uint32_t nm = slot_nm(pb), ne = slot_ne(pb);
@@ -694,64 +771,23 @@ __device__ inline uint32_t finalize_pe(const DevIndex& ix, const MapParamsDev& P
     const uint32_t n_frag_slots = ps.n_fragments + 1;     // + the (empty, no rescue) extra entry
     constexpr uint32_t MAX_PAIRS = 64;
     double pair_score[MAX_PAIRS]; int64_t pair_dist[MAX_PAIRS]; uint8_t pair_c0[MAX_PAIRS], pair_c1[MAX_PAIRS], pair_better[MAX_PAIRS];
-    uint32_t n_pairs = 0; bool found_pair = false;
-    uint8_t unpaired[2 * MAX_CANDS]; uint32_t n_unpaired = 0;
-    uint32_t status = GB_ITEM_OK;
-#pragma unroll 1
-    for (uint32_t f = 0; f < n_frag_slots && status == GB_ITEM_OK; f++) {
-        bool has0 = false, has1 = false;
-#pragma unroll 1
-        for (uint32_t c = 0; c < cl.n; c++) if (cl.frag[c] == f) { if (cl.read[c] == 0) has0 = true; else has1 = true; }
-        if (has0 && has1) {
-            found_pair = true;
-#pragma unroll 1
-            for (uint32_t c0 = 0; c0 < cl.n && status == GB_ITEM_OK; c0++) {
-                if (cl.frag[c0] != f || cl.read[c0] != 0) continue;
-#pragma unroll 1
-                for (uint32_t c1 = 0; c1 < cl.n; c1++) {
-                    if (cl.frag[c1] != f || cl.read[c1] != 1) continue;
-                    if (n_pairs >= MAX_PAIRS) { status = GB_ITEM_OUT_FULL; break; }
-                    // distance_between(aln1, aln2): initial_position(aln1) -> final_position(aln2) (:3895-3903)
-                    const PathBuf p0 = slot_buf(cand_base, cl.slot[c0], map_cap, edit_cap);
-                    const PathBuf p1 = slot_buf(cand_base, cl.slot[c1], map_cap, edit_cap);
-                    int64_t dist = 0;
-                    {
-                        const gb_mapping first = p0.maps[0];
-                        const uint32_t nm1 = slot_nm(p1), ne1 = slot_ne(p1);
-                        const gb_mapping last = p1.maps[nm1 - 1];
-                        uint32_t used = 0;
-#pragma unroll 1
-                        for (uint32_t x = ne1 - last.n_edits; x < ne1; x++) { const uint32_t wd = p1.edits[x]; const uint32_t op = wd & 3u; if (op != GB_EDIT_INS) used += (op == GB_EDIT_SUB) ? 1u : (wd >> 4); }
-                        dist = oriented_distance(ix, first.node, first.offset, last.node, (uint32_t)last.offset + used);
-                    }
-                    // score_alignment_pair (:6017-6028)
-                    const double dev = (double)dist - a.frag_mean;
-                    const double ll = (-dev * dev / (2.0 * a.frag_sd * a.frag_sd)) / P.log_base;
-                    const double sc_sum = (double)cl.score[c0] + (double)cl.score[c1] + ll;
-                    const double worse = fmin((double)cl.score[c0], (double)cl.score[c1]);
-                    pair_score[n_pairs] = fmax(sc_sum, worse); pair_dist[n_pairs] = dist;
-                    pair_c0[n_pairs] = (uint8_t)c0; pair_c1[n_pairs] = (uint8_t)c1; pair_better[n_pairs] = ps.better_cluster_count[f];
-                    n_pairs++;
-                }
-            }
-        } else {
-#pragma unroll 1
-            for (uint32_t r = 0; r < 2; r++) for (uint32_t c = 0; c < cl.n; c++) if (cl.frag[c] == f && cl.read[c] == r) unpaired[n_unpaired++] = (uint8_t)c;
-        }
-    }
-    if (status != GB_ITEM_OK) return status;
+    uint32_t n_pairs, n_unpaired; bool found_pair;
+    uint8_t unpaired[2 * MAX_CANDS];
+    auto frag_of = [&](uint32_t c) { return (uint32_t)cl.frag[c]; };
+    auto read_of = [&](uint32_t c) { return (uint32_t)cl.read[c]; };
+    auto score_of = [&](uint32_t c) { return cl.score[c]; };
+    auto dist_of = [&](uint32_t c0, uint32_t c1) {
+        return distance_between(ix, slot_buf(cand_base, cl.slot[c0], map_cap, edit_cap), slot_buf(cand_base, cl.slot[c1], map_cap, edit_cap));
+    };
+    if (!collect_pairs<MAX_PAIRS>(cl.n, n_frag_slots, frag_of, read_of, score_of, dist_of, ps.better_cluster_count, a.frag_mean, a.frag_sd, P.log_base,
+                                  pair_score, pair_dist, pair_c0, pair_c1, pair_better, n_pairs, found_pair, unpaired, n_unpaired))
+        return GB_ITEM_OUT_FULL;
     if (n_unpaired > 0 && P.max_rescue_attempts != 0) return GB_ITEM_RETRY;     // needs mate rescue: the rescue kernel redoes this pair
 
     if (n_unpaired > 0 && !found_pair) {
-        // max_rescue_attempts == 0 (:2227-2287): best alignment of each end, MAPQ 1
-        int best_c[2] = {-1, -1}; int32_t best_score[2] = {0, 0};
-#pragma unroll 1
-        for (uint32_t u = 0; u < n_unpaired; u++) {
-            const uint32_t c = unpaired[u]; const uint32_t r = cl.read[c];
-            bool beats = cl.score[c] > best_score[r];
-            if (!beats && cl.score[c] == best_score[r]) beats = (rng_next(rng) % 2) != 0;
-            if (beats) { best_c[r] = (int)c; best_score[r] = cl.score[c]; }
-        }
+        // max_rescue_attempts == 0 (:2237-2287): best alignment of each end, MAPQ 1
+        int best_c[2]; int32_t best_score[2];
+        best_unpaired_per_end(unpaired, n_unpaired, read_of, score_of, rng, best_c, best_score);
 #pragma unroll 1
         for (uint32_t r = 0; r < 2; r++) {
             out[r].mapq = 1;
@@ -769,22 +805,13 @@ __device__ inline uint32_t finalize_pe(const DevIndex& ix, const MapParamsDev& P
 
     // winner (:2505-2598)
     uint8_t po[MAX_PAIRS];
-#pragma unroll 1
-    for (uint32_t p = 0; p < n_pairs; p++) { uint32_t j = p; while (j > 0 && pair_score[p] > pair_score[po[j - 1]]) { po[j] = po[j - 1]; j--; } po[j] = (uint8_t)p; }
-    {
-        uint32_t ties = 0;
-#pragma unroll 1
-        while (ties < n_pairs && !(pair_score[po[0]] > pair_score[po[ties]])) ties++;
-#pragma unroll 1
-        for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = po[j]; po[j] = po[i]; po[i] = t; }
-    }
+    sort_shuffling_ties(n_pairs, [&](uint32_t x, uint32_t y) { return pair_score[x] > pair_score[y]; }, po, rng);
     double scores_sorted[MAX_PAIRS];
 #pragma unroll 1
     for (uint32_t p = 0; p < n_pairs; p++) scores_sorted[p] = pair_score[po[p]];
     const uint32_t wp = po[0];
     const double uncapped_mapq = scores_sorted[0] == 0 ? 0.0 : max_mapping_quality(scores_sorted, n_pairs, P.log_base);
-    double fragment_cluster_cap = INFINITY;
-    if (pair_better[wp] > 1) fragment_cluster_cap = -10.0 * log10(1.0 - (1.0 / (double)pair_better[wp]));
+    const double cluster_cap = fragment_cluster_cap(pair_better[wp]);
     double caps[2] = {0.0, 0.0};
     double* cbuf = reinterpret_cast<double*>(dps.Hp);
     uint64_t* ordbuf = reinterpret_cast<uint64_t*>(dps.Hc);
@@ -793,17 +820,10 @@ __device__ inline uint32_t finalize_pe(const DevIndex& ix, const MapParamsDev& P
     const uint32_t cwin[2] = {pair_c0[wp], pair_c1[wp]};
 #pragma unroll 1
     for (uint32_t r = 0; r < 2; r++) {
-        const double escape_bonus = uncapped_mapq < 2147483647.0 ? 1.0 : 2.0;
-        const double mapq_cap = fmin(fragment_cluster_cap, (caps[0] + caps[1]) * escape_bonus);
-        double capped = fmin(mapq_cap, uncapped_mapq);
-        if (pair_dist[wp] == INT64_MAX) capped = capped / 2.0;
-        double read_mapq = fmax(fmin(capped, 120.0) / 2.0, 0.0);
         PathBuf pb = slot_buf(cand_base, cl.slot[cwin[r]], map_cap, edit_cap);
         const uint32_t nm = slot_nm(pb), ne = slot_ne(pb);
-        if (nm == 0) read_mapq = 0;
         out[r].score = cl.score[cwin[r]]; out[r].flags |= nm ? GB_ALN_MAPPED : 0; out[r].n_mappings = (uint16_t)nm; out[r].n_edits = ne;
-        out[r].mapq = (uint8_t)(int32_t)read_mapq;
-        out[r].mapq_uncapped = (float)uncapped_mapq; out[r].mapq_explored_cap = (float)mapq_cap;
+        pair_read_mapq(uncapped_mapq, cluster_cap, caps[0] + caps[1], pair_dist[wp] == INT64_MAX, INFINITY, out[r]);
         if (lane == 0) write_alignment(ix, pb, nm, ne, sread[r], L[r], r == 1, out_maps[r], out_edits[r]);
     }
     __syncwarp();

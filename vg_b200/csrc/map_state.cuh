@@ -60,6 +60,24 @@ __device__ __forceinline__ void rng_skip(DevRng& r, uint32_t n) {
     r.state = minstd_mulmod(r.state, minstd_pow(n));
 }
 
+// sort_shuffling_ties (utility.hpp:770-793): order = 0 .. n - 1 stably sorted by `before(a, b)` (a goes first), then the
+// items tied with the first are shuffled with the LazyRNG (deterministic_shuffle: one draw per tied item after the first).
+template <typename Before>
+__device__ __forceinline__ void sort_shuffling_ties(uint32_t n, Before before, uint8_t* order, DevRng& rng) {
+#pragma unroll 1
+    for (uint32_t c = 0; c < n; c++) {
+        uint32_t j = c;
+#pragma unroll 1
+        while (j > 0 && before(c, order[j - 1])) { order[j] = order[j - 1]; j--; }
+        order[j] = (uint8_t)c;
+    }
+    uint32_t ties = 0;
+#pragma unroll 1
+    while (ties < n && !before(order[0], order[ties])) ties++;
+#pragma unroll 1
+    for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = order[j]; order[j] = order[i]; order[i] = t; }
+}
+
 // One minimizer of the read in SCORE order (MinimizerMapper::Minimizer, minimizer_mapper.hpp:565).
 struct __align__(16) DevMinimizer {
     uint64_t hash;

@@ -392,26 +392,6 @@ __device__ inline int32_t attempt_rescue(const DevIndex& ix, const MapParamsDev&
     return score;
 }
 
-// maximum_mapping_quality_exact with multiplicities (mapping_quality_calculator.cpp:26-67); returns the int32-truncated value
-__device__ inline double max_mapping_quality_mult(const double* scores, uint32_t n, double log_base, const double* mult) {
-    const double quality_scale_factor = 10.0 / log(10.0);
-    double log_sum_exp = -DBL_MAX, to_score = -DBL_MAX;
-#pragma unroll 1
-    for (int64_t i = (int64_t)n - 1; i >= 0; --i) {
-        double score = log_base * scores[i];
-        if (score >= to_score) to_score = score;
-        if (mult && mult[i] > 1.0) score += log(mult[i]);
-        log_sum_exp = d_add_log(log_sum_exp, score);
-    }
-    if (n == 1) {
-        if (mult && mult[0] <= 1.0) log_sum_exp = d_add_log(log_sum_exp, 0.0);
-        else if (!mult) log_sum_exp = d_add_log(log_sum_exp, 0.0);
-    }
-    const double direct = -quality_scale_factor * d_subtract_log(0.0, to_score - log_sum_exp);
-    const double mq = isinf(direct) ? 2147483647.0 : direct;
-    return (double)(int32_t)mq;
-}
-
 constexpr uint32_t RESCUE_MAX_PAIRS = 96;
 enum : uint8_t { PT_PAIRED = 0, PT_UNPAIRED = 1, PT_RESCUED_FROM_FIRST = 2, PT_RESCUED_FROM_SECOND = 3 };
 
@@ -429,91 +409,49 @@ __device__ inline uint32_t finalize_pe_rescue(const DevIndex& ix, const MapParam
         out[r].read_id = read_idx0 + r; out[r].score = 0; out[r].mapq = 0; out[r].flags = GB_ALN_PAIRED; out[r].n_mappings = 0; out[r].n_edits = 0;
         out[r].mapq_uncapped = 0.f; out[r].mapq_explored_cap = 0.f;
     }
-    const uint32_t n_frag_slots = ps.n_fragments + 1;
     const uint32_t rescue_frag = ps.n_fragments;               // alignments.back(): the fragment that collects rescued alignments
     double pair_score[RESCUE_MAX_PAIRS]; int64_t pair_dist[RESCUE_MAX_PAIRS];
     uint8_t pair_c0[RESCUE_MAX_PAIRS], pair_c1[RESCUE_MAX_PAIRS], pair_better[RESCUE_MAX_PAIRS], pair_type[RESCUE_MAX_PAIRS];
-    uint32_t n_pairs = 0; bool found_pair = false;
-    uint8_t unpaired[2 * MAX_CANDS]; uint32_t n_unpaired = 0;
-    uint32_t unpaired_count[2] = {0, 0}, rescued_count[2] = {0, 0};
+    uint32_t n_pairs, n_unpaired; bool found_pair;
+    uint8_t unpaired[2 * MAX_CANDS];
     uint32_t status = GB_ITEM_OK;
     int32_t best_alignment_scores[2] = {0, 0};
 #pragma unroll 1
     for (uint32_t c = 0; c < cl.n; c++) best_alignment_scores[cl.read[c]] = max(best_alignment_scores[cl.read[c]], cl.score[c]);
-    // distance_between(first mate's alignment c0, second mate's alignment c1) (:3895-3903)
-    auto distance_between = [&](uint32_t c0, uint32_t c1) -> int64_t {
-        const PathBuf p0 = slot_buf(cand_base, cl.slot[c0], map_cap, edit_cap);
-        const PathBuf p1 = slot_buf(cand_base, cl.slot[c1], map_cap, edit_cap);
-        const gb_mapping first = p0.maps[0];
-        const uint32_t nm1 = slot_nm(p1), ne1 = slot_ne(p1);
-        const gb_mapping last = p1.maps[nm1 - 1];
-        uint32_t used = 0;
-#pragma unroll 1
-        for (uint32_t x = ne1 - last.n_edits; x < ne1; x++) { const uint32_t wd = p1.edits[x]; const uint32_t op = wd & 3u; if (op != GB_EDIT_INS) used += (op == GB_EDIT_SUB) ? 1u : (wd >> 4); }
-        return oriented_distance(ix, first.node, first.offset, last.node, (uint32_t)last.offset + used);
+    auto frag_of = [&](uint32_t c) { return (uint32_t)cl.frag[c]; };
+    auto read_of = [&](uint32_t c) { return (uint32_t)cl.read[c]; };
+    auto score_of = [&](uint32_t c) { return cl.score[c]; };
+    // distance_between(first mate's alignment c0, second mate's alignment c1)
+    auto dist_of = [&](uint32_t c0, uint32_t c1) {
+        return distance_between(ix, slot_buf(cand_base, cl.slot[c0], map_cap, edit_cap), slot_buf(cand_base, cl.slot[c1], map_cap, edit_cap));
     };
-    auto score_alignment_pair = [&](int32_t s0, int32_t s1, int64_t dist) -> double {
-        const double dev = (double)dist - a.frag_mean;
-        const double ll = (-dev * dev / (2.0 * a.frag_sd * a.frag_sd)) / P.log_base;
-        return fmax((double)s0 + (double)s1 + ll, fmin((double)s0, (double)s1));
-    };
+    // the fragments of the clusters: rescue_frag is still empty
+    if (!collect_pairs<RESCUE_MAX_PAIRS>(cl.n, rescue_frag, frag_of, read_of, score_of, dist_of, ps.better_cluster_count, a.frag_mean, a.frag_sd, P.log_base,
+                                         pair_score, pair_dist, pair_c0, pair_c1, pair_better, n_pairs, found_pair, unpaired, n_unpaired))
+        return GB_ITEM_OUT_FULL;
 #pragma unroll 1
-    for (uint32_t f = 0; f + 1 < n_frag_slots && status == GB_ITEM_OK; f++) {
-        bool has0 = false, has1 = false;
+    for (uint32_t p = 0; p < n_pairs; p++) pair_type[p] = PT_PAIRED;
+    // per end: the unpaired alignments and their scores (the MAPQ cap of an unpaired winner)
+    uint32_t unpaired_count[2] = {0, 0}, rescued_count[2] = {0, 0};
+    double unpaired_scores[2][2 * MAX_CANDS];
 #pragma unroll 1
-        for (uint32_t c = 0; c < cl.n; c++) if (cl.frag[c] == f) { if (cl.read[c] == 0) has0 = true; else has1 = true; }
-        if (has0 && has1) {
-            found_pair = true;
-#pragma unroll 1
-            for (uint32_t c0 = 0; c0 < cl.n && status == GB_ITEM_OK; c0++) {
-                if (cl.frag[c0] != f || cl.read[c0] != 0) continue;
-#pragma unroll 1
-                for (uint32_t c1 = 0; c1 < cl.n; c1++) {
-                    if (cl.frag[c1] != f || cl.read[c1] != 1) continue;
-                    if (n_pairs >= RESCUE_MAX_PAIRS) { status = GB_ITEM_OUT_FULL; break; }
-                    const int64_t dist = distance_between(c0, c1);
-                    pair_score[n_pairs] = score_alignment_pair(cl.score[c0], cl.score[c1], dist); pair_dist[n_pairs] = dist;
-                    pair_c0[n_pairs] = (uint8_t)c0; pair_c1[n_pairs] = (uint8_t)c1; pair_better[n_pairs] = ps.better_cluster_count[f]; pair_type[n_pairs] = PT_PAIRED;
-                    n_pairs++;
-                }
-            }
-        } else {
-#pragma unroll 1
-            for (uint32_t r = 0; r < 2; r++) for (uint32_t c = 0; c < cl.n; c++) if (cl.frag[c] == f && cl.read[c] == r) { unpaired[n_unpaired++] = (uint8_t)c; unpaired_count[r]++; }
-        }
-    }
-    if (status != GB_ITEM_OK) return status;
+    for (uint32_t u = 0; u < n_unpaired; u++) { const uint32_t c = unpaired[u], r = cl.read[c]; unpaired_scores[r][unpaired_count[r]++] = (double)cl.score[c]; }
 
-    double unpaired_scores[2][2 * MAX_CANDS]; uint32_t n_unpaired_scores[2] = {0, 0};
     if (n_unpaired > 0) {
         if (!found_pair) {
-            int best_c[2] = {-1, -1}; int32_t best_score[2] = {0, 0};
-#pragma unroll 1
-            for (uint32_t u = 0; u < n_unpaired; u++) {
-                const uint32_t c = unpaired[u]; const uint32_t r = cl.read[c];
-                unpaired_scores[r][n_unpaired_scores[r]++] = (double)cl.score[c];
-                bool beats = cl.score[c] > best_score[r];
-                if (!beats && cl.score[c] == best_score[r]) beats = (rng_next(rng) % 2) != 0;
-                if (beats) { best_c[r] = (int)c; best_score[r] = cl.score[c]; }
-            }
+            int best_c[2]; int32_t best_score[2];
+            best_unpaired_per_end(unpaired, n_unpaired, read_of, score_of, rng, best_c, best_score);
             if (best_score[0] != 0 && best_score[1] != 0) {
                 // the best alignments of the two ends as an (unpaired) pair at "infinite" distance (:2288-2334)
-                pair_score[n_pairs] = score_alignment_pair(cl.score[best_c[0]], cl.score[best_c[1]], INT64_MAX); pair_dist[n_pairs] = INT64_MAX;
+                pair_score[n_pairs] = score_alignment_pair(cl.score[best_c[0]], cl.score[best_c[1]], INT64_MAX, a.frag_mean, a.frag_sd, P.log_base);
+                pair_dist[n_pairs] = INT64_MAX;
                 pair_c0[n_pairs] = (uint8_t)best_c[0]; pair_c1[n_pairs] = (uint8_t)best_c[1]; pair_better[n_pairs] = 0; pair_type[n_pairs] = PT_UNPAIRED;
                 n_pairs++;
             }
         }
         // rescue from the unpaired alignments, best first (:2338-2457)
         uint8_t uo[2 * MAX_CANDS];
-#pragma unroll 1
-        for (uint32_t u = 0; u < n_unpaired; u++) { uint32_t j = u; while (j > 0 && cl.score[unpaired[u]] > cl.score[unpaired[uo[j - 1]]]) { uo[j] = uo[j - 1]; j--; } uo[j] = (uint8_t)u; }
-        {
-            uint32_t ties = 0;
-#pragma unroll 1
-            while (ties < n_unpaired && !(cl.score[unpaired[uo[0]]] > cl.score[unpaired[uo[ties]]])) ties++;
-#pragma unroll 1
-            for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = uo[j]; uo[j] = uo[i]; uo[i] = t; }
-        }
+        sort_shuffling_ties(n_unpaired, [&](uint32_t x, uint32_t y) { return cl.score[unpaired[x]] > cl.score[unpaired[y]]; }, uo, rng);
         uint32_t unskipped = 0;
 #pragma unroll 1
         for (uint32_t oi = 0; oi < n_unpaired && status == GB_ITEM_OK; oi++) {
@@ -537,7 +475,10 @@ __device__ inline uint32_t finalize_pe_rescue(const DevIndex& ix, const MapParam
             const uint32_t cr = cl.n;
             cl.score[cr] = rescued_score; cl.slot[cr] = (uint8_t)slot; cl.frag[cr] = (uint8_t)rescue_frag; cl.read[cr] = (uint8_t)other; cl.n++;
             int64_t dist; double score;
-            if (pb.n_maps != 0) { dist = r == 0 ? distance_between(c, cr) : distance_between(cr, c); score = score_alignment_pair(cl.score[c], rescued_score, dist); }
+            if (pb.n_maps != 0) {
+                dist = r == 0 ? dist_of(c, cr) : dist_of(cr, c);
+                score = score_alignment_pair(cl.score[c], rescued_score, dist, a.frag_mean, a.frag_sd, P.log_base);
+            }
             else { score = (double)cl.score[c]; dist = INT64_MAX; }
             pair_score[n_pairs] = score; pair_dist[n_pairs] = dist;
             pair_c0[n_pairs] = (uint8_t)(r == 0 ? c : cr); pair_c1[n_pairs] = (uint8_t)(r == 0 ? cr : c);
@@ -550,15 +491,7 @@ __device__ inline uint32_t finalize_pe_rescue(const DevIndex& ix, const MapParam
 
     // winner (:2505-2598)
     uint8_t po[RESCUE_MAX_PAIRS];
-#pragma unroll 1
-    for (uint32_t p = 0; p < n_pairs; p++) { uint32_t j = p; while (j > 0 && pair_score[p] > pair_score[po[j - 1]]) { po[j] = po[j - 1]; j--; } po[j] = (uint8_t)p; }
-    {
-        uint32_t ties = 0;
-#pragma unroll 1
-        while (ties < n_pairs && !(pair_score[po[0]] > pair_score[po[ties]])) ties++;
-#pragma unroll 1
-        for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = po[j]; po[j] = po[i]; po[i] = t; }
-    }
+    sort_shuffling_ties(n_pairs, [&](uint32_t x, uint32_t y) { return pair_score[x] > pair_score[y]; }, po, rng);
     double scores_sorted[RESCUE_MAX_PAIRS], mult[RESCUE_MAX_PAIRS];
     double est_mult[2];
 #pragma unroll 1
@@ -573,9 +506,8 @@ __device__ inline uint32_t finalize_pe_rescue(const DevIndex& ix, const MapParam
         else mult[p] = est_mult[t == PT_RESCUED_FROM_FIRST ? 0 : 1];
     }
     const uint32_t wp = po[0];
-    const double uncapped_mapq = scores_sorted[0] == 0 ? 0.0 : max_mapping_quality_mult(scores_sorted, n_pairs, P.log_base, all_rescued ? mult : nullptr);
-    double fragment_cluster_cap = INFINITY;
-    if (pair_better[wp] > 1) fragment_cluster_cap = -10.0 * log10(1.0 - (1.0 / (double)pair_better[wp]));
+    const double uncapped_mapq = scores_sorted[0] == 0 ? 0.0 : max_mapping_quality(scores_sorted, n_pairs, P.log_base, all_rescued ? mult : nullptr);
+    const double cluster_cap = fragment_cluster_cap(pair_better[wp]);
     double caps[2] = {0.0, 0.0};
     double* cbuf = reinterpret_cast<double*>(dps.Hp);
     uint64_t* ordbuf = reinterpret_cast<uint64_t*>(dps.Hc);
@@ -584,19 +516,12 @@ __device__ inline uint32_t finalize_pe_rescue(const DevIndex& ix, const MapParam
     const uint32_t cwin[2] = {pair_c0[wp], pair_c1[wp]};
 #pragma unroll 1
     for (uint32_t r = 0; r < 2; r++) {
-        const double escape_bonus = uncapped_mapq < 2147483647.0 ? 1.0 : 2.0;
-        double mapq_cap = fmin(fragment_cluster_cap, (caps[0] + caps[1]) * escape_bonus);
-        if (pair_type[wp] == PT_UNPAIRED) mapq_cap = fmin(mapq_cap, max_mapping_quality(unpaired_scores[r], n_unpaired_scores[r], P.log_base));   // :2735-2739
-        double capped = fmin(mapq_cap, uncapped_mapq);
-        if (pair_dist[wp] == INT64_MAX) capped = capped / 2.0;
-        double read_mapq = fmax(fmin(capped, 120.0) / 2.0, 0.0);
         PathBuf pb = slot_buf(cand_base, cl.slot[cwin[r]], map_cap, edit_cap);
         const uint32_t nm = slot_nm(pb), ne = slot_ne(pb);
-        if (nm == 0) read_mapq = 0;
         out[r].score = cl.score[cwin[r]]; out[r].flags |= nm ? GB_ALN_MAPPED : 0; out[r].n_mappings = (uint16_t)nm; out[r].n_edits = ne;
         if (cl.frag[cwin[r]] == rescue_frag) out[r].flags |= GB_ALN_RESCUED;
-        out[r].mapq = (uint8_t)(int32_t)read_mapq;
-        out[r].mapq_uncapped = (float)uncapped_mapq; out[r].mapq_explored_cap = (float)mapq_cap;
+        const double unpaired_cap = pair_type[wp] == PT_UNPAIRED ? max_mapping_quality(unpaired_scores[r], unpaired_count[r], P.log_base) : INFINITY;   // :2735-2739
+        pair_read_mapq(uncapped_mapq, cluster_cap, caps[0] + caps[1], pair_dist[wp] == INT64_MAX, unpaired_cap, out[r]);
         if (lane == 0 && nm) write_alignment(ix, pb, nm, ne, sread[r], L[r], r == 1, out_maps[r], out_edits[r]);
     }
     __syncwarp();

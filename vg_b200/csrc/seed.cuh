@@ -810,21 +810,7 @@ __device__ __forceinline__ uint32_t cluster_phase_se(const DevIndex& ix, const M
         auto comes_before = [&](uint32_t a, uint32_t b) {
             return (sm.c_cov[a] > sm.c_cov[b]) || (sm.c_cov[a] == sm.c_cov[b] && sm.c_score[a] > sm.c_score[b]);
         };
-#pragma unroll 1
-        for (uint32_t c = 0; c < Cn; c++) {
-            uint32_t j = c;
-#pragma unroll 1
-            while (j > 0 && comes_before(c, sm.c_order[j - 1])) { sm.c_order[j] = sm.c_order[j - 1]; j--; }
-            sm.c_order[j] = (uint8_t)c;
-        }
-        uint32_t ties = 0;
-#pragma unroll 1
-        while (ties < Cn && !comes_before(sm.c_order[0], sm.c_order[ties])) ties++;
-#pragma unroll 1
-        for (uint32_t i = 1; i < ties; i++) {
-            const uint32_t j = rng_next(rng) % (i + 1);
-            const uint8_t t = sm.c_order[j]; sm.c_order[j] = sm.c_order[i]; sm.c_order[i] = t;
-        }
+        sort_shuffling_ties(Cn, comes_before, sm.c_order, rng);
         const double cutoff = Cn == 0 ? 0.0 : sm.c_cov[sm.c_order[0]] - P.cluster_coverage_threshold;
         uint32_t unskipped = 0, kept_cluster_count = 0;
 #pragma unroll 1
@@ -1055,15 +1041,7 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
             }
             // better_cluster_count (:1657-1690)
             auto total = [&](uint32_t f) { return (fc[0][f] + fc[1][f]) + (fs[0][f] + fs[1][f]); };
-#pragma unroll 1
-            for (uint32_t f = 0; f < n_frag; f++) { uint32_t j = f; while (j > 0 && total(f) > total(fo[j - 1])) { fo[j] = fo[j - 1]; j--; } fo[j] = (uint8_t)f; }
-            {
-                uint32_t ties = 0;
-#pragma unroll 1
-                while (ties < n_frag && !(total(fo[0]) > total(fo[ties]))) ties++;
-#pragma unroll 1
-                for (uint32_t i = 1; i < ties; i++) { const uint32_t j = rng_next(rng) % (i + 1); const uint8_t t = fo[j]; fo[j] = fo[i]; fo[i] = t; }
-            }
+            sort_shuffling_ties(n_frag, [&](uint32_t x, uint32_t y) { return total(x) > total(y); }, fo, rng);
             double prev_score_sum = 0.0;
             uint8_t* better = gps->better_cluster_count;
 #pragma unroll 1

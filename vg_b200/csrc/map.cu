@@ -73,7 +73,7 @@ seed_kernel(DevIndex ix, MapParamsDev P, MapBatch b, SeedPools pools) {
         const bool work = active && status == GB_ITEM_OK;
         DevRng rng; rng.inited = 0; rng.state = 0; rng.seed = 0;
         if (work) {
-            for (uint32_t i = lane; i < L; i += 32) sm.read[i] = b.reads[rb + i];
+            stage_read(sm.read, b.reads + rb, L);
             __syncwarp();
             rng.seed = fold_seed(0u, sm.read, L);                     // LazyRNG seed: the read sequence (:620-622)
             status = seed_phase_a(ix, P, sm, L, pools, rng, rs);

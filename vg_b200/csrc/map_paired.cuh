@@ -41,7 +41,11 @@ __global__ void __launch_bounds__(SEED_WARPS * 32, SEED_BLOCKS_PER_SM)
 seed_kernel_pe(DevIndex ix, MapParamsDev P, MapBatch b, SeedPools pools, PairBatch pb) {
     extern __shared__ __align__(16) uint8_t smem[];
     __shared__ uint32_t s_base;
+    // The two reads' states live from phase A to the end of the round: in registers they would take 32 of the 64.
+    __shared__ ReadState s_rs[SEED_WARPS][2];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    ReadState& rs0 = s_rs[warp][0];
+    ReadState& rs1 = s_rs[warp][1];
     const uint32_t lay_L = LC ? (uint32_t)LC : b.Lc, lay_M = MC ? (uint32_t)MC : b.Mc, lay_C = CC ? (uint32_t)CC : b.Cc;
     const SeedSmem sm = carve_seed_smem(smem + (size_t)warp * seed_smem_bytes(lay_L, lay_M, lay_C), lay_L, lay_M, lay_C, b.Ns);
     const uint32_t n_pairs = b.n_reads / 2;
@@ -55,57 +59,44 @@ seed_kernel_pe(DevIndex ix, MapParamsDev P, MapBatch b, SeedPools pools, PairBat
         if (base >= limit) break;
         const bool active = base + warp < limit;
         const uint32_t p = !active ? 0u : (b.in_list ? b.in_list[base + warp] : base + warp);
-        ReadState rs0, rs1;
-        memset(&rs0, 0, sizeof(ReadState)); memset(&rs1, 0, sizeof(ReadState));
+        if (lane < 2 * sizeof(ReadState) / 4) reinterpret_cast<uint32_t*>(s_rs[warp])[lane] = 0;
+        __syncwarp();
         uint32_t n_fragments = 0;
         uint32_t status = GB_ITEM_OK;
-        uint32_t L[2] = {0, 0};
+        // read offsets and lengths are loaded again where they are used (L1 hits) rather than held through the phases
+        auto read_len = [&](uint32_t r) { return (uint32_t)(b.read_off[2 * p + r + 1] - b.read_off[2 * p + r]); };
+        DevRng rng; rng.inited = 0; rng.state = 0; rng.seed = 0;
         if (active) {
-#pragma unroll 1
-            for (uint32_t r = 0; r < 2; r++) L[r] = (uint32_t)(b.read_off[2 * p + r + 1] - b.read_off[2 * p + r]);
-            if (L[0] > b.Lc || L[1] > b.Lc) status = GB_ITEM_OUT_FULL;
+            const uint64_t rb0 = b.read_off[2 * p], rb1 = b.read_off[2 * p + 1];
+            const uint32_t L0 = (uint32_t)(rb1 - rb0), L1 = (uint32_t)(b.read_off[2 * p + 2] - rb1);
+            if (L0 > b.Lc || L1 > b.Lc) status = GB_ITEM_OUT_FULL;
+            // LazyRNG seed: aln1.sequence() + aln2.sequence() with mate 2 already rightward (:1529-1531)
+            else rng.seed = fold_seed(fold_seed(0u, b.reads + rb0, L0), b.reads + rb1, L1);
         }
         const bool work = active && status == GB_ITEM_OK;
-        // LazyRNG seed: aln1.sequence() + aln2.sequence() with mate 2 already rightward (:1529-1531)
-        DevRng rng; rng.inited = 0; rng.state = 0; rng.seed = 0;
-        if (work) {
-#pragma unroll 1
-            for (uint32_t r = 0; r < 2; r++) {
-                const uint64_t rb = b.read_off[2 * p + r];
-#pragma unroll 1
-                for (uint32_t i = lane; i < L[r]; i += 32) sm.read[i] = b.reads[rb + i];
-                __syncwarp();
-                rng.seed = fold_seed(rng.seed, sm.read, L[r]);
-                __syncwarp();
-            }
-        }
 #pragma unroll 1
         for (uint32_t r = 0; r < 2; r++) {
             __syncthreads();
             if (work && status == GB_ITEM_OK) {
-                const uint64_t rb = b.read_off[2 * p + r];
-#pragma unroll 1
-                for (uint32_t i = lane; i < L[r]; i += 32) sm.read[i] = b.reads[rb + i];
+                const uint32_t Lr = read_len(r);
+                stage_read(sm.read, b.reads + b.read_off[2 * p + r], Lr);
                 __syncwarp();
-                ReadState cur;
-                memset(&cur, 0, sizeof(ReadState));
-                status = seed_phase_a(ix, P, sm, L[r], pools, rng, cur);
-                if (r) rs1 = cur; else rs0 = cur;
+                status = seed_phase_a(ix, P, sm, Lr, pools, rng, s_rs[warp][r]);
                 __syncwarp();
             }
         }
         __syncthreads();
         if (work && status == GB_ITEM_OK)
-            status = cluster_phase_pe(ix, P, sm, L[0], L[1], 2 * p, pb.fragment_limit, pools, rng, rs0, rs1, pb.pairs + p, n_fragments);
+            status = cluster_phase_pe(ix, P, sm, read_len(0), read_len(1), 2 * p, pb.fragment_limit, pools, rng, rs0, rs1, pb.pairs + p, n_fragments);
         if (!active) continue;
         if (status == GB_ITEM_RETRY) {
             if (lane == 0) b.retry_list[atomicAdd(b.retry_count, 1u)] = p;
             continue;
         }
-        rs0.rng = rng; rs1.rng = rng;
-        rs0.status = rs1.status = status;
-        if (status != GB_ITEM_OK) { rs0.item_cnt = rs1.item_cnt = 0; }
         if (lane == 0) {
+            rs0.rng = rng; rs1.rng = rng;
+            rs0.status = rs1.status = status;
+            if (status != GB_ITEM_OK) { rs0.item_cnt = rs1.item_cnt = 0; }
             b.states[2 * p] = rs0; b.states[2 * p + 1] = rs1;
             // cluster_phase_pe fills the record when the pair has clusters
             if (status != GB_ITEM_OK || n_fragments == 0) { pb.pairs[p].n_fragments = 0; pb.pairs[p].found_paired_cluster = 0; }

@@ -145,17 +145,33 @@ __device__ __forceinline__ uint32_t pow13(uint32_t e) {
     return r;
 }
 
-// seedNumber = fold(seed * 13 + byte) over `bytes` (utility.cpp:911-927), continuing from `seed`.
+// seedNumber = fold(seed * 13 + byte) over `bytes` (utility.cpp:911-927), continuing from `seed`: byte i weighs 13^(L-1-i).
+// Lane q takes the bytes q, q + 32, ... places from the end (Horner in 13^32, then times 13^q), so its loads are
+// independent of each other and `bytes` can be the read in HBM.
 __device__ inline uint32_t fold_seed(uint32_t seed, const uint8_t* bytes, uint32_t L) {
-    const int lane = lane_id();
-    const uint32_t chunk = (L + 31) / 32;
-    const uint32_t b = min(L, lane * chunk), e = min(L, b + chunk);
-    uint32_t fold = 0;
-    for (uint32_t i = b; i < e; i++) fold = fold * 13u + bytes[i];
-    uint32_t term = fold * pow13(L - e);
+    const uint32_t lane = lane_id();
+    constexpr uint32_t P32 = 0x6a265881u;                        // 13^32 mod 2^32
+    const int32_t n = L > lane ? (int32_t)((L - 1 - lane) >> 5) + 1 : 0;
+    uint32_t acc = 0;
+#pragma unroll 4
+    for (int32_t j = n - 1; j >= 0; j--) acc = acc * P32 + bytes[L - 1 - lane - 32 * (uint32_t)j];
+    uint32_t term = acc * pow13(lane);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) term += __shfl_xor_sync(FULL, term, o);
     return seed * pow13(L) + term;
+}
+
+// Copy a read of L bytes to shared memory with up to 256 bytes of loads in flight per round trip (L <= 256 takes one).
+__device__ __forceinline__ void stage_read(uint8_t* dst, const uint8_t* src, uint32_t L) {
+    const uint32_t lane = lane_id();
+#pragma unroll 1
+    for (uint32_t base = 0; base < L; base += 256) {
+        uint32_t v[8];
+#pragma unroll
+        for (uint32_t k = 0; k < 8; k++) { const uint32_t i = base + lane + 32 * k; v[k] = i < L ? src[i] : 0u; }
+#pragma unroll
+        for (uint32_t k = 0; k < 8; k++) { const uint32_t i = base + lane + 32 * k; if (i < L) dst[i] = (uint8_t)v[k]; }
+    }
 }
 
 // set bits [lo, hi) of a bitmap made of 32-bit words
@@ -445,9 +461,25 @@ __device__ __forceinline__ uint32_t seed_phase_a(const DevIndex& ix, const MapPa
             }
         }
         __syncwarp();
-        if (lane == 0) {
+        // When no minimizer has more than hit_cap hits, the hit-cap||score-fraction clause passes every minimizer that
+        // reaches it, so the target score is never lowered and the running state cannot change a decision: passing is
+        // hits > 0 && run hits <= hard_hit_cap, one position per lane.
+        const bool use_fraction = (P.hit_cap != 0 || P.minimizer_score_fraction != 1.0);
+        bool over_cap = false;
+#pragma unroll 1
+        for (uint32_t i = lane; i < M; i += 32) over_cap |= s_hits[i] > P.hit_cap;
+        if (!use_fraction || !__any_sync(FULL, over_cap)) {
+            uint32_t hits_sum = 0;
+#pragma unroll 1
+            for (uint32_t i = lane; i < M; i += 32) {
+                const uint32_t hits = s_hits[i];
+                const bool passing = hits > 0 && (s_runhits[i] & 0x7fffffffu) <= P.hard_hit_cap;
+                sm.m_pass[i] = passing ? 1 : 0;
+                hits_sum += passing ? hits : 0u;
+            }
+            total_hits = (uint32_t)warp_sum((int)hits_sum);
+        } else if (lane == 0) {
             double base_target_score = 0.0, target_score = 0.0, selected_score = 0.0;
-            const bool use_fraction = (P.hit_cap != 0 || P.minimizer_score_fraction != 1.0);
             if (use_fraction) {
                 for (uint32_t i = 0; i < M; i++) base_target_score += s_score[i];
                 target_score = (base_target_score * P.minimizer_score_fraction) + 0.000001;
@@ -622,9 +654,7 @@ struct ClusterScratch {
     uint32_t* startbits;   // [16]   k-mer start bitmap of one cluster (coverage)
     double* fs0; double* fs1; double* fc0; double* fc1;   // [F] per-fragment best score / coverage per read
     uint32_t* side;        // [2 * Cc] fragment label of each read cluster
-    uint32_t* heads;       // [2 * Cc]
     uint8_t* fo;           // [F]
-    uint8_t* has_first;    // [F]
     uint8_t* has_pair;     // [F]
     uint32_t F;
     // joint clustering of small seed sets in shared memory (whatever is left of the dead arrays)
@@ -634,7 +664,7 @@ struct ClusterScratch {
     uint32_t ns_cap;       // <= 64
 };
 __host__ __device__ inline uint32_t cluster_scratch_fragments(uint32_t Cc) { return 2 * Cc < MAX_FRAGMENTS ? 2 * Cc : MAX_FRAGMENTS; }
-__host__ __device__ inline size_t cluster_scratch_bytes(uint32_t Cc) { const size_t F = cluster_scratch_fragments(Cc); return 64 + 32 * F + 16 * (size_t)Cc + 3 * F; }
+__host__ __device__ inline size_t cluster_scratch_bytes(uint32_t Cc) { const size_t F = cluster_scratch_fragments(Cc); return 64 + 32 * F + 8 * (size_t)Cc + 2 * F; }
 __host__ __device__ inline size_t seed_dead_bytes(uint32_t Lc, uint32_t Mc) { return (size_t)Lc * 16 + (size_t)Mc * 24; }
 __device__ __forceinline__ ClusterScratch carve_cluster_scratch(const SeedSmem& sm) {
     ClusterScratch cs;
@@ -643,8 +673,8 @@ __device__ __forceinline__ ClusterScratch carve_cluster_scratch(const SeedSmem& 
     cs.startbits = (uint32_t*)p; p += 64;
     cs.fs0 = (double*)p; p += 8 * cs.F; cs.fs1 = (double*)p; p += 8 * cs.F;
     cs.fc0 = (double*)p; p += 8 * cs.F; cs.fc1 = (double*)p; p += 8 * cs.F;
-    cs.side = (uint32_t*)p; p += 8 * sm.Cc; cs.heads = (uint32_t*)p; p += 8 * sm.Cc;
-    cs.fo = p; p += cs.F; cs.has_first = p; p += cs.F; cs.has_pair = p; p += cs.F;
+    cs.side = (uint32_t*)p; p += 8 * sm.Cc;
+    cs.fo = p; p += cs.F; cs.has_pair = p; p += cs.F;
     const size_t used = ((size_t)(p - reinterpret_cast<uint8_t*>(sm.khash)) + 15) & ~(size_t)15;
     const size_t dead = seed_dead_bytes(sm.Lc, sm.Mc);
     cs.ns_cap = dead > used ? (uint32_t)min((size_t)min(64u, sm.ns_max), (dead - used) / 18) : 0u;
@@ -738,16 +768,21 @@ __device__ __forceinline__ uint32_t emit_items(const DevIndex& ix, const SeedSme
     if (n_kept == 0) return GB_ITEM_OK;
     uint32_t item_off = 0;
     if (!pool_claim(pools.item_cursor, n_kept, pools.item_cap, pools.overflow, item_off)) return GB_ITEM_OUT_FULL;
+    // one ext_seeds range for the whole read, the items' seeds back to back in kept order
+    uint32_t total = 0;
+#pragma unroll 1
+    for (uint32_t t = 0; t < n_kept; t++) {
+        const uint32_t label = sm.c_label[cbase + kept[t]];
+#pragma unroll 1
+        for (uint32_t i = lane; i < H; i += 32) total += seeds[i].label == label ? 1u : 0u;
+    }
+    total = (uint32_t)warp_sum((int)total);
+    uint32_t eoff = 0;
+    if (!pool_claim(pools.ext_cursor, total, pools.ext_cap, pools.overflow, eoff)) return GB_ITEM_OUT_FULL;
 #pragma unroll 1
     for (uint32_t t = 0; t < n_kept; t++) {
         const uint32_t c = kept[t];
         const uint32_t label = sm.c_label[cbase + c];
-        uint32_t cnt = 0;
-#pragma unroll 1
-        for (uint32_t i = lane; i < H; i += 32) cnt += seeds[i].label == label ? 1u : 0u;
-        cnt = (uint32_t)warp_sum((int)cnt);
-        uint32_t eoff = 0;
-        if (!pool_claim(pools.ext_cursor, cnt, pools.ext_cap, pools.overflow, eoff)) return GB_ITEM_OUT_FULL;
         uint32_t wpos = 0;
 #pragma unroll 1
         for (uint32_t base = 0; base < H; base += 32) {
@@ -764,12 +799,13 @@ __device__ __forceinline__ uint32_t emit_items(const DevIndex& ix, const SeedSme
             wpos += __popc(bal);
         }
         if (lane == 0) {
-            DevItem it; it.read = read_idx; it.seed_off = eoff; it.seed_cnt = cnt;
+            DevItem it; it.read = read_idx; it.seed_off = eoff; it.seed_cnt = wpos;
             it.fragment = sm.c_frag[cbase + c] | (cflags ? (uint32_t)cflags[c] << 8 : 0u);         // deferred selection flags, see cluster_phase_pe
 #pragma unroll
             for (uint32_t x = 0; x < PRESENT_WORDS; x++) it.present[x] = sm.c_present[(cbase + c) * PRESENT_WORDS + x];
             pools.items[item_off + t] = it;
         }
+        eoff += wpos;
     }
     item_off_out = item_off;
     return GB_ITEM_OK;
@@ -846,9 +882,10 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
                                                      const SeedPools& pools, DevRng& rng, ReadState& rs0, ReadState& rs1, PairState* gps,
                                                      uint32_t& n_fragments_out) {
     const int lane = lane_id();
-    DevSeed* s0 = pools.seeds + rs0.seed_off; DevSeed* s1 = pools.seeds + rs1.seed_off;
+    // the records' bases are read again from the states at each use rather than held in registers through the phase
+    auto seeds_of = [&](uint32_t r) { return pools.seeds + (r ? rs1.seed_off : rs0.seed_off); };
     const uint32_t H0 = rs0.seed_cnt, H1 = rs1.seed_cnt;
-    const DevMinimizer* m0 = pools.minimizers + rs0.min_off; const DevMinimizer* m1 = pools.minimizers + rs1.min_off;
+    auto mins_of = [&](uint32_t r) -> const DevMinimizer* { return pools.minimizers + (r ? rs1.min_off : rs0.min_off); };
     n_fragments_out = 0;
     if (H0 + H1 == 0) return GB_ITEM_OK;
     const int32_t read_limit = (int32_t)max(P.distance_limit, L0 + 50);
@@ -863,39 +900,49 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
         // over the masks; labels live in shared memory.
 #pragma unroll 1
         for (uint32_t i = lane; i < n_all; i += 32) {
-            const DevSeed sd = i < H0 ? s0[i] : s1[i - H0];
+            const DevSeed sd = i < H0 ? seeds_of(0)[i] : seeds_of(1)[i - H0];
             cs.seedbuf[i] = make_uint4(sd.id_off, (uint32_t)sd.c_in, (uint32_t)sd.c_out, sd.slot);
         }
         __syncwarp();
-        uint4 own[2]; bool has[2]; uint64_t adj_f[2] = {0, 0}, adj_r[2] = {0, 0};
+        bool has[2]; uint64_t adj_f[2] = {0, 0}, adj_r[2] = {0, 0};
 #pragma unroll
-        for (uint32_t q = 0; q < 2; q++) { const uint32_t i = lane + 32 * q; has[q] = i < n_all; own[q] = has[q] ? cs.seedbuf[i] : make_uint4(0, 0, 0, 0); }
-        // unoriented minimum distance through the payload, as seeds_within; INT_MAX when unreachable
-        auto seed_dist = [&ix](const uint4& a, const uint4& c) -> int32_t {
-            if ((a.x >> 10) == (c.x >> 10)) { const int32_t d = (int32_t)(c.x & 1023u) - (int32_t)(a.x & 1023u); return d >= 0 ? d : -d; }
-            if (a.w < c.w) return (int32_t)c.y - (int32_t)a.z;
-            if (c.w < a.w) return (int32_t)a.y - (int32_t)c.z;
-            return same_site_distance(ix, a.x, (int32_t)a.y, (int32_t)a.z, c.x, (int32_t)c.y, (int32_t)c.z);
+        for (uint32_t q = 0; q < 2; q++) has[q] = lane + 32 * q < n_all;
+        // The distance is unoriented, so the relations are symmetric: lane q walks row q over every column and row q + 32
+        // over the columns >= 32; the columns < 32 of rows >= 32 are read back from the first rows by vote.  Pairs of
+        // different nodes in one site need the site table (same_site_distance, out of line): they are set aside in
+        // `pend` and resolved after the walk, so the call and the registers it saves stay off the row loop.
+        auto add_edge = [&](uint32_t row, uint32_t j, int32_t d, uint64_t& af, uint64_t& ar) {
+            if (d <= fragment_limit) af |= 1ull << j;
+            if (d <= read_limit && (row < H0) == (j < H0)) ar |= 1ull << j;
         };
-        // rows of seeds 0..31: lane i walks all j
-        for (uint32_t j = 0; j < n_all; j++) {
-            const uint4 sj = cs.seedbuf[j];
-            if (!has[0] || (uint32_t)lane == j) continue;
-            const int32_t d = seed_dist(own[0], sj);
-            if (d == INT_MAX) continue;
-            if (d <= fragment_limit) adj_f[0] |= 1ull << j;
-            if (d <= read_limit && ((uint32_t)lane < H0) == (j < H0)) adj_r[0] |= 1ull << j;
-        }
-        // rows of the few seeds beyond 32: the warp evaluates one row at a time, lane = column, rows by vote
+        auto walk_row = [&](uint32_t row, uint32_t j0, uint64_t& af, uint64_t& ar) {
+            const uint4 a = row < n_all ? cs.seedbuf[row] : make_uint4(0, 0, 0, 0);
+            uint64_t pend = 0;
+#pragma unroll 1
+            for (uint32_t j = j0; j < n_all; j++) {
+                const uint4 c = cs.seedbuf[j];
+                if (row >= n_all || row == j) continue;
+                int32_t d;
+                if ((a.x >> 10) == (c.x >> 10)) { d = (int32_t)(c.x & 1023u) - (int32_t)(a.x & 1023u); d = d >= 0 ? d : -d; }
+                else if (a.w < c.w) d = (int32_t)c.y - (int32_t)a.z;
+                else if (c.w < a.w) d = (int32_t)a.y - (int32_t)c.z;
+                else { pend |= 1ull << j; continue; }
+                add_edge(row, j, d, af, ar);
+            }
+#pragma unroll 1
+            while (pend) {
+                const uint32_t j = (uint32_t)(__ffsll((long long)pend) - 1); pend &= pend - 1;
+                const uint4 c = cs.seedbuf[j];
+                const int32_t d = same_site_distance(ix, a.x, (int32_t)a.y, (int32_t)a.z, c.x, (int32_t)c.y, (int32_t)c.z);
+                if (d != INT_MAX) add_edge(row, j, d, af, ar);
+            }
+        };
+        walk_row(lane, 0, adj_f[0], adj_r[0]);
+        if (n_all > 32) walk_row(lane + 32, 32, adj_f[1], adj_r[1]);
 #pragma unroll 1
         for (uint32_t i = 32; i < n_all; i++) {
-            const uint4 si = cs.seedbuf[i];
-            bool f_lo = false, r_lo = false, f_hi = false, r_hi = false;
-            if (has[0]) { const int32_t d = seed_dist(si, own[0]); f_lo = d <= fragment_limit && d != INT_MAX; r_lo = d <= read_limit && d != INT_MAX && ((uint32_t)lane < H0) == (i < H0); }
-            if (has[1] && lane + 32 != (int)i) { const int32_t d = seed_dist(si, own[1]); f_hi = d <= fragment_limit && d != INT_MAX; r_hi = d <= read_limit && d != INT_MAX && ((uint32_t)lane + 32 < H0) == (i < H0); }
-            const uint64_t row_f = (uint64_t)__ballot_sync(FULL, f_lo) | ((uint64_t)__ballot_sync(FULL, f_hi) << 32);
-            const uint64_t row_r = (uint64_t)__ballot_sync(FULL, r_lo) | ((uint64_t)__ballot_sync(FULL, r_hi) << 32);
-            if ((uint32_t)lane + 32 == i) { adj_f[1] = row_f; adj_r[1] = row_r; }
+            const uint32_t lo_f = __ballot_sync(FULL, (adj_f[0] >> i) & 1ull), lo_r = __ballot_sync(FULL, (adj_r[0] >> i) & 1ull);
+            if ((uint32_t)lane + 32 == i) { adj_f[1] |= lo_f; adj_r[1] |= lo_r; }
         }
 #pragma unroll 1
         for (uint32_t level = 0; level < 2; level++) {
@@ -939,7 +986,7 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
         // read-cluster labels back to the records (local index space of each read)
 #pragma unroll 1
         for (uint32_t i = lane; i < n_all; i += 32) {
-            if (i < H0) s0[i].label = cs.lab_read[i]; else s1[i - H0].label = (uint32_t)cs.lab_read[i] - H0;
+            if (i < H0) seeds_of(0)[i].label = cs.lab_read[i]; else seeds_of(1)[i - H0].label = (uint32_t)cs.lab_read[i] - H0;
         }
         __syncwarp();
 #pragma unroll 1
@@ -963,26 +1010,26 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
         // the upper bits of `source` (source < 128); passes 1, 2: the read clusters of each read.
 #pragma unroll 1
         for (uint32_t pass = 0; pass < 3; pass++) {
-            DevSeed* sa = pass == 2 ? s1 : s0; const uint32_t na = pass == 2 ? H1 : H0;
+            DevSeed* sa = seeds_of(pass == 2); const uint32_t na = pass == 2 ? H1 : H0;
             const uint32_t nb = pass == 0 ? H1 : 0u;
 #pragma unroll 1
             for (uint32_t i = lane; i < na; i += 32) sa[i].label = i;
 #pragma unroll 1
-            for (uint32_t i = lane; i < nb; i += 32) s1[i].label = na + i;
+            for (uint32_t i = lane; i < nb; i += 32) seeds_of(1)[i].label = na + i;
             __syncwarp();
-            propagate_labels(ix, sa, na, s1, nb, pass == 0 ? fragment_limit : read_limit);
+            propagate_labels(ix, sa, na, seeds_of(1), nb, pass == 0 ? fragment_limit : read_limit);
             if (pass == 0) {
 #pragma unroll 1
-                for (uint32_t i = lane; i < H0; i += 32) s0[i].source |= s0[i].label << 8;
+                for (uint32_t i = lane; i < H0; i += 32) seeds_of(0)[i].source |= seeds_of(0)[i].label << 8;
 #pragma unroll 1
-                for (uint32_t i = lane; i < H1; i += 32) s1[i].source |= s1[i].label << 8;
+                for (uint32_t i = lane; i < H1; i += 32) seeds_of(1)[i].source |= seeds_of(1)[i].label << 8;
             }
             __syncwarp();
         }
         // the fragment label of each read-cluster root goes to the side table, then `source` is restored
 #pragma unroll 1
         for (uint32_t r = 0; r < 2; r++) {
-            DevSeed* sr = r ? s1 : s0; const uint32_t Hr = r ? H1 : H0;
+            DevSeed* sr = seeds_of(r); const uint32_t Hr = r ? H1 : H0;
             uint32_t n_roots = 0;
 #pragma unroll 1
             for (uint32_t base = 0; base < Hr && !overflow; base += 32) {
@@ -1001,7 +1048,7 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
     }
 #pragma unroll 1
     for (uint32_t r = 0; r < 2 && !overflow; r++) {
-        const uint32_t cn = collect_clusters(sm, cs, r ? s1 : s0, r ? H1 : H0, r ? m1 : m0, r ? rs1.min_cnt : rs0.min_cnt, ix.k, r ? L1 : L0, r * sm.Cc);
+        const uint32_t cn = collect_clusters(sm, cs, seeds_of(r), r ? H1 : H0, mins_of(r), r ? rs1.min_cnt : rs0.min_cnt, ix.k, r ? L1 : L0, r * sm.Cc);
         if (cn == 0xffffffffu) overflow = 1;
         else if (r) Cn[1] = cn; else Cn[0] = cn;
     }
@@ -1014,31 +1061,60 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
     uint32_t n_kept0 = 0, n_kept1 = 0, defer_ties = 0;
     uint32_t status = GB_ITEM_OK;
     uint32_t n_frag = 0;
-    if (lane == 0) {
-        // fragment renumbering (:129-141 of the clusterer wrapper)
+    {
+        // fragment renumbering (:129-141 of the clusterer wrapper): fragments are numbered in order of first appearance
+        // over read 1's clusters, then read 2's.  Lane g takes cluster g of that concatenation (n_cl <= 2 * Cc <= 32 *
+        // PRESENT_WORDS); its fragment id is the number of first appearances before its head's first cluster.
+        const uint32_t n_cl = Cn[0] + Cn[1];
+        auto slot = [&](uint32_t g) { return g < Cn[0] ? g : sm.Cc + g - Cn[0]; };
+        uint32_t first_pos[PRESENT_WORDS], firstw[PRESENT_WORDS];
+#pragma unroll
+        for (uint32_t t = 0; t < PRESENT_WORDS; t++) {
+            const uint32_t g = lane + 32 * t;
+            uint32_t fp = g;
+            if (g < n_cl) {
+                const uint32_t head = cs.side[slot(g)];
 #pragma unroll 1
-        for (uint32_t r = 0; r < 2; r++) for (uint32_t c = 0; c < (r ? Cn[1] : Cn[0]); c++) {
-            const uint32_t head = cs.side[r * sm.Cc + c];
-            uint32_t f = 0; while (f < n_frag && cs.heads[f] != head) f++;
-            if (f == n_frag) cs.heads[n_frag++] = head;
-            sm.c_frag[r * sm.Cc + c] = (uint8_t)f;
-        }
-        if (n_frag > cs.F) status = table_full(sm.Cc, MAX_CLUSTERS);
-        else {
-            double* const fs[2] = {cs.fs0, cs.fs1}; double* const fc[2] = {cs.fc0, cs.fc1};
-            uint8_t* has_first = cs.has_first; uint8_t* has_pair = cs.has_pair; uint8_t* fo = cs.fo;
-#pragma unroll 1
-            for (uint32_t f = 0; f < n_frag; f++) { has_first[f] = has_pair[f] = 0; fs[0][f] = fs[1][f] = fc[0][f] = fc[1][f] = 0.0; }
-            bool found_paired_cluster = false;
-#pragma unroll 1
-            for (uint32_t c = 0; c < Cn[0]; c++) has_first[sm.c_frag[c]] = 1;
-#pragma unroll 1
-            for (uint32_t c = 0; c < Cn[1]; c++) { const uint32_t f = sm.c_frag[sm.Cc + c]; has_pair[f] = has_first[f]; if (has_first[f]) found_paired_cluster = true; }
-#pragma unroll 1
-            for (uint32_t r = 0; r < 2; r++) for (uint32_t c = 0; c < (r ? Cn[1] : Cn[0]); c++) {
-                const uint32_t t = r * sm.Cc + c, f = sm.c_frag[t];
-                fs[r][f] = max(fs[r][f], sm.c_score[t]); fc[r][f] = max(fc[r][f], sm.c_cov[t]);
+                for (uint32_t x = 0; x < g; x++) if (cs.side[slot(x)] == head) { fp = x; break; }
             }
+            first_pos[t] = fp;
+            firstw[t] = __ballot_sync(FULL, g < n_cl && fp == g);
+            n_frag += __popc(firstw[t]);
+        }
+#pragma unroll
+        for (uint32_t t = 0; t < PRESENT_WORDS; t++) {
+            const uint32_t g = lane + 32 * t, fp = first_pos[t];
+            if (g < n_cl) {
+                uint32_t f = 0;
+#pragma unroll
+                for (uint32_t x = 0; x < PRESENT_WORDS; x++)
+                    f += __popc(firstw[x] & (x < (fp >> 5) ? 0xffffffffu : x == (fp >> 5) ? (1u << (fp & 31)) - 1u : 0u));
+                sm.c_frag[slot(g)] = (uint8_t)f;
+            }
+        }
+        __syncwarp();
+    }
+    if (n_frag > cs.F) status = table_full(sm.Cc, MAX_CLUSTERS);
+    else {
+        // per-fragment best score and coverage of each read, and whether both reads have a cluster in it: lane f scans the clusters
+        bool any_pair = false;
+#pragma unroll 1
+        for (uint32_t f = lane; f < n_frag; f += 32) {
+            bool hf = false, hp = false;
+            double bs0 = 0.0, bs1 = 0.0, bc0 = 0.0, bc1 = 0.0;
+#pragma unroll 1
+            for (uint32_t c = 0; c < Cn[0]; c++) if (sm.c_frag[c] == f) { hf = true; bs0 = max(bs0, sm.c_score[c]); bc0 = max(bc0, sm.c_cov[c]); }
+#pragma unroll 1
+            for (uint32_t c = sm.Cc; c < sm.Cc + Cn[1]; c++) if (sm.c_frag[c] == f) { hp = hf; bs1 = max(bs1, sm.c_score[c]); bc1 = max(bc1, sm.c_cov[c]); }
+            cs.has_pair[f] = hp;
+            cs.fs0[f] = bs0; cs.fs1[f] = bs1; cs.fc0[f] = bc0; cs.fc1[f] = bc1;
+            any_pair |= hp;
+        }
+        const bool found_paired_cluster = __any_sync(FULL, any_pair);
+        __syncwarp();
+        if (lane == 0) {
+            double* const fs[2] = {cs.fs0, cs.fs1}; double* const fc[2] = {cs.fc0, cs.fc1};
+            uint8_t* has_pair = cs.has_pair; uint8_t* fo = cs.fo;
             // better_cluster_count (:1657-1690)
             auto total = [&](uint32_t f) { return (fc[0][f] + fc[1][f]) + (fs[0][f] + fs[1][f]); };
             sort_shuffling_ties(n_frag, [&](uint32_t x, uint32_t y) { return total(x) > total(y); }, fo, rng);
@@ -1145,7 +1221,7 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
         uint32_t item_off = 0;
         const uint32_t nk = r ? n_kept1 : n_kept0;
         dbg_dump_clusters(pools, sm, read_idx0 + r, r * sm.Cc, r ? Cn[1] : Cn[0], r ? kept1 : kept0, nk, r && defer_ties);
-        const uint32_t st = emit_items(ix, sm, pools, r ? s1 : s0, r ? H1 : H0, r ? m1 : m0, read_idx0 + r, r ? kept1 : kept0, nk, r * sm.Cc, item_off,
+        const uint32_t st = emit_items(ix, sm, pools, seeds_of(r), r ? H1 : H0, mins_of(r), read_idx0 + r, r ? kept1 : kept0, nk, r * sm.Cc, item_off,
                                        r && defer_ties ? cflags1 : nullptr);
         if (st != GB_ITEM_OK) return st;
         if (r) { rs1.item_off = item_off; rs1.item_cnt = nk; } else { rs0.item_off = item_off; rs0.item_cnt = nk; }

@@ -10,38 +10,16 @@ import numpy as np
 import pytest
 
 import helpers as H
+from test_emit import ABSENT, MAPPED, PAIRED, RESCUED, SEC, _build, _corner_batch, _dv_sweep, _hand_graph, _host, _names_t, _reads
 from vg_b200 import capi, synth
 
 pytestmark = pytest.mark.gpu
-
-MAPPED, SEC, PAIRED, RESCUED, ABSENT = capi.GB_ALN_MAPPED, capi.GB_ALN_SECONDARY, capi.GB_ALN_PAIRED, capi.GB_ALN_RESCUED, capi.GB_ALN_ABSENT
 
 
 def _t(a, dtype=None):
     import torch
     a = np.ascontiguousarray(a if dtype is None else a.astype(dtype))
     return torch.from_numpy(a.view(np.uint8).reshape(-1).copy() if dtype is None else a.copy()).cuda()
-
-
-def _names_t(names):
-    enc = [s.encode() for s in names]
-    off = np.concatenate([[0], np.cumsum([len(b) for b in enc])]).astype(np.int64)
-    return np.frombuffer(b"".join(enc) + b"\0", dtype=np.uint8).copy(), off
-
-
-def _host(kind, view, aln, maps, edits, rbuf, qbuf, read_off, names=None, cap=None):
-    """gb_emit_gaf / gb_emit_gam into a buffer of `cap` bytes (default: generous for short reads)."""
-    lib = capi.load_library()
-    fn = {"gaf": lib.gb_emit_gaf, "gam": lib.gb_emit_gam}[kind]
-    nbuf, noff = _names_t(names) if names is not None else (None, None)
-    aln = np.ascontiguousarray(aln)
-    cap = cap or 4096 + len(aln) * 4096
-    out = np.zeros(cap, dtype=np.uint8); used = C.c_uint64()
-    rc = fn(C.byref(view), len(aln), capi.ptr(aln), capi.ptr(maps), len(maps), capi.ptr(edits), len(edits), len(read_off) - 1, capi.ptr(rbuf),
-            capi.ptr(qbuf) if qbuf is not None else None, capi.ptr(read_off), capi.ptr(nbuf) if nbuf is not None else None,
-            capi.ptr(noff) if noff is not None else None, capi.ptr(out), cap, C.byref(used))
-    assert rc == capi.GB_OK, rc
-    return out[: used.value].tobytes()
 
 
 def _device(dev, kind, aln, maps, edits, rbuf, qbuf, read_off, names=None):
@@ -173,62 +151,10 @@ def test_records_straight_from_map_batch_device():
 
 
 # ---- hand-made records -------------------------------------------------------------------------------------------------
-def _build(recs):
-    """recs: [(read_id, flags, score, [(oriented node, offset, [(op "MSID", length, base)...])...])] -> aln, maps, edits."""
-    n = len(recs)
-    cols = {k: np.zeros(n, dtype=capi.alignment_dt[k]) for k in capi.alignment_dt.names}
-    mnode, moff, mne, words = [], [], [], []
-    for x, (rid, flags, score, mp) in enumerate(recs):
-        cols["read_id"][x] = rid; cols["flags"][x] = flags; cols["score"][x] = score
-        cols["mapping_off"][x] = len(mnode); cols["edit_off"][x] = len(words); cols["n_mappings"][x] = len(mp)
-        for node, off, eds in mp:
-            mnode.append(node); moff.append(off); mne.append(len(eds))
-            words.extend((ln << 4) | (b << 2) | "MSID".index(op) for op, ln, b in eds)
-        cols["n_edits"][x] = len(words) - cols["edit_off"][x]
-    cols["mapq"][:] = np.arange(n) % 61
-    cols["mapq_uncapped"][:] = np.arange(n, dtype=np.float32) * 0.37
-    cols["mapq_explored_cap"][:] = np.where(np.arange(n) % 3 == 0, np.inf, np.arange(n) * 1.5)
-    aln = np.zeros(n, dtype=capi.alignment_dt)
-    for k, v in cols.items():
-        aln[k] = v
-    maps = np.zeros(len(mnode) + 1, dtype=capi.mapping_dt)
-    maps["node"][:-1] = mnode; maps["offset"][:-1] = moff; maps["n_edits"][:-1] = mne
-    return aln, maps, np.array(words + [0], dtype=np.uint32)
-
-
-def _hand_graph():
-    rng = np.random.default_rng(12)
-    seqs = ["".join("ACGT"[c] for c in rng.integers(0, 4, size=1000)) for _ in range(3)]
-    return capi.HostIndex(seqs, [[2, 4, 6]], None, k=15, w=5)
-
-
-def _reads(lengths, seed=5, n_frac=0.0):
-    rng = np.random.default_rng(seed)
-    reads = [bytes(synth.BASES[rng.integers(0, 4, size=ln)]) for ln in lengths]
-    if n_frac:
-        reads = [bytes(ord("N") if rng.random() < n_frac else c for c in r) for r in reads]
-    rbuf, _, read_off = H.pack_reads(reads)
-    qbuf = (np.arange(len(rbuf)) % 41).astype(np.uint8)
-    return rbuf, qbuf, read_off
-
-
 def test_hand_made_formatting_corners():
     index = _hand_graph()
     dev = capi.Device(index, 0)
-    rbuf, qbuf, read_off = _reads([40, 40, 20, 0, 25000, 30001, 40, 40], n_frac=0.05)
-    recs = [
-        (0, MAPPED, 31, [(2, 5, [("I", 4, 0), ("M", 30, 0), ("S", 1, 2), ("M", 5, 0)])]),                  # leading soft clip
-        (1, MAPPED, -17, [(3, 990, [("M", 10, 0)]), (6, 0, [("I", 7, 0)]), (4, 0, [("D", 12, 0), ("M", 23, 0)])]),  # insertion-only mapping, <id
-        (2, MAPPED, -2147483648, [(4, 0, [("I", 20, 0)])]),                                                  # all-insertion path: '*'
-        (3, 0, 0, []),                                                                                       # empty read, unmapped
-        (4, MAPPED | SEC, 5, [(2, 0, [("M", 1000, 0)])] * 25 + [(4, 0, [("D", 1, 0)])]),                      # dv 1/25001: exponent form
-        (5, MAPPED | RESCUED, 77, [(2, 0, [("M", 1000, 0)])] * 30 + [(4, 0, [("M", 1, 0), ("D", 2, 0)])]),    # dv 2/30003
-        (6, MAPPED | PAIRED, 0, [(2, 0, [("M", 39, 0), ("S", 1, 1)])]),
-        (7, PAIRED | RESCUED, 9, []),
-        (6, ABSENT, 0, []),
-        (0, MAPPED, 1, [(2, 0, []), (2, 5, [("I", 4, 0), ("M", 36, 0)])]),                                   # a mapping without edits
-    ]
-    aln, maps, edits = _build(recs)
+    rbuf, qbuf, read_off, recs, aln, maps, edits = _corner_batch()
     gaf = _host("gaf", index.view, aln, maps, edits, rbuf, qbuf, read_off, cap=1 << 22).decode().splitlines()
     assert gaf[2].split("\t")[5] == "*" and "AS:i:-2147483648" in gaf[2]
     assert re.search(r"\tdv:f:[1-9](\.\d+)?e-05(\t|$)", gaf[4]) and re.search(r"\tdv:f:6\.6\d*e-05(\t|$)", gaf[5])
@@ -267,32 +193,11 @@ def test_gam_group_boundaries(n_present):
 
 
 def test_dv_matches_printf_g6_over_a_dense_range():
-    """one record per (matches, block): every pair with block <= 1100, and long deletions with block up to ~3e5; the dv:f
-    field must read as Python's '%.6g' % (1.0 - m / b), which is correctly rounded like glibc."""
+    """every (matches, block) pair with block <= 1100 and long deletions (test_emit._dv_sweep): the dv:f field must read as
+    Python's '%.6g' % (1.0 - m / b), which is correctly rounded like glibc."""
     index = _hand_graph()
     dev = capi.Device(index, 0)
-    B = 1100
-    large_m = [10007, 24999, 99999, 123457, 299990]
-    large_d = [1, 2, 3, 7, 19, 29, 30, 31, 97, 500, 999]
-    rbuf, _, read_off = _reads(list(range(B + 1)) + large_m)
-    recs, want = [], []
-    for b in range(1, B + 1):
-        for m in range(b + 1):
-            ins = b - m
-            m1, m2 = min(m, 1000), m - min(m, 1000)
-            if m == 0:
-                mp = [(2, 0, [("I", ins, 0)])]
-            elif m2 == 0:
-                mp = [(2, 0, [("M", m1, 0)] + ([("I", ins, 0)] if ins else []))]
-            else:
-                mp = [(2, 0, [("M", m1, 0)]), (4, 0, [("M", m2, 0)] + ([("I", ins, 0)] if ins else []))]
-            recs.append((b, MAPPED, 0, mp)); want.append("%.6g" % (1.0 - m / b))
-    for j, m in enumerate(large_m):
-        for d in large_d:
-            mp = [(2, 0, [("M", 1000, 0)])] * (m // 1000) + [(4, 0, [("M", m % 1000, 0)])] + [(6, 0, [("D", d, 0)])]
-            recs.append((B + 1 + j, MAPPED, 0, mp)); want.append("%.6g" % (1.0 - m / (m + d)))
-    assert sum("e-" in w for w in want) >= 10
-    aln, maps, edits = _build(recs)
+    rbuf, read_off, (aln, maps, edits), want = _dv_sweep()
     got = _device(dev, "gaf", aln, maps, edits, rbuf, None, read_off).decode()
     dv = [line.rsplit("\tdv:f:", 1)[1] for line in got.splitlines()]
     bad = [(i, g, w) for i, (g, w) in enumerate(zip(dv, want)) if g != w]

@@ -201,6 +201,37 @@ int gb_index_build_with_hits(uint32_t n_node_ids, const uint8_t* node_seq, const
                              const gb_dist_payload* dist, uint32_t k, uint32_t w,
                              uint64_t n_hits, const uint64_t* keys, const uint64_t* positions,
                              gb_host_index** out);
+/* gb_index_from_gbz and gb_index_build_from_gbwt with the minimizer step on CUDA device `device_ordinal`: the same GBZ reader,
+ * record validation, sequences, distance payload, GBWT blob and table placement on the host; on the GPU one warp per start node
+ * follows the GBWT search states to every haplotype-consistent continuation of k + w - 2 bases, computes the minimizers of each
+ * start node + continuation string, and radix-sorts and de-duplicates the (key, position) pairs.  The result is byte-identical to
+ * the host entry point's: every gb_index_view array, k, w, n_paths, gb_index_save's file, gb_index_has_distance_model.
+ * Synchronous; every device allocation is freed before the call returns.  Argument checks come first and return the host entry
+ * point's codes (GB_ERR_ARG for NULL path / out / node arrays, k == 0, k > 31, w == 0, and for device_ordinal < 0 or out of
+ * range); then GB_ERR_NO_DEVICE without a GPU (there is no host fallback: the host entry points are the CPU route); then the
+ * host entry point's GB_ERR_FORMAT for a damaged file or record.  With keys / positions given, gb_index_build_from_gbwt_device
+ * takes the table from them as the host call does and enumerates nothing.  GB_ERR_CAPACITY, beyond the host's cases, when a
+ * GBWT record has more than 2^31 - 1 visits, when the longest node + k + w - 2 bases (16 B each) do not fit one warp's shared
+ * memory, or when one start node has more minimizers than the pair pool holds.
+ * HBM: the node records (32 B per node id), both sequence orientations (2 B per base), the GBWT blob, 20 B per start node,
+ * the warps' search-state stacks (16 B per warp x the largest GBWT record, about the haplotype count; at most 256 MiB) and the
+ * pair pool with its sort buffers (56 B per pair, at most 2 GiB: min(2 GiB, 56 B x the pairs before de-duplication)).
+ * Start nodes are processed in batches whose pairs fit the pool; GIRAFFE_B200_INDEX_POOL_PAIRS (a pair count; for tests
+ * only) shrinks the pool so that a small graph needs several batches. */
+int gb_index_from_gbz_device(const char* path, uint32_t k, uint32_t w, int device_ordinal, gb_host_index** out);
+int gb_index_build_from_gbwt_device(uint32_t n_node_ids, const uint8_t* node_seq, const uint64_t* node_off, uint32_t n_paths,
+                                    const uint32_t* gbwt_words, uint64_t n_words, const uint32_t* rec_off,
+                                    const gb_dist_payload* dist, uint32_t k, uint32_t w,
+                                    uint64_t n_hits, const uint64_t* keys, const uint64_t* positions,
+                                    int device_ordinal, gb_host_index** out);
+/* How a build spent its time, host-clocked (seconds), and what its minimizer step visited: start nodes and continuations of the
+ * window enumeration (0 for the haplotype scan and for a table given by the caller), (key, position) pairs before and after
+ * de-duplication.  All zero for an index read by gb_index_load. */
+typedef struct gb_index_timing {
+    double sequences_s, distance_s, gbwt_s, minimizers_s, table_s;
+    uint64_t start_nodes, continuations, raw_pairs, unique_pairs;
+} gb_index_timing;
+int gb_index_build_timing(const gb_host_index* ix, gb_index_timing* out);
 int gb_index_save(const gb_flat_index* ix, const char* path);
 int gb_index_load(const char* path, gb_host_index** out);
 

@@ -55,6 +55,11 @@ class FlatIndex(C.Structure):
     ]
 
 
+class IndexTiming(C.Structure):
+    _fields_ = [(name, C.c_double) for name in ("sequences_s", "distance_s", "gbwt_s", "minimizers_s", "table_s")] + \
+               [(name, C.c_uint64) for name in ("start_nodes", "continuations", "raw_pairs", "unique_pairs")]
+
+
 class Scores(C.Structure):
     _fields_ = [("match", C.c_int8), ("mismatch", C.c_int8), ("gap_open", C.c_int8),
                 ("gap_extend", C.c_int8), ("full_length_bonus", C.c_int8)]
@@ -146,6 +151,9 @@ def load_library() -> C.CDLL:
         "gb_index_from_gbz_min": (st, [C.c_char_p, C.c_char_p, C.c_char_p, vp]),
         "gb_index_build_with_hits": (st, [u32, vp, vp, u32, vp, vp, vp, u32, u32, u64, vp, vp, vp]),
         "gb_index_build_from_gbwt": (st, [u32, vp, vp, u32, vp, u64, vp, vp, u32, u32, u64, vp, vp, vp]),
+        "gb_index_from_gbz_device": (st, [C.c_char_p, u32, u32, C.c_int, vp]),
+        "gb_index_build_from_gbwt_device": (st, [u32, vp, vp, u32, vp, u64, vp, vp, u32, u32, u64, vp, vp, C.c_int, vp]),
+        "gb_index_build_timing": (st, [vp, C.POINTER(IndexTiming)]),
         "gb_index_save": (st, [fix, C.c_char_p]),
         "gb_index_load": (st, [C.c_char_p, vp]),
         "gb_set_scores": (st, [vp, C.POINTER(Scores)]),
@@ -324,16 +332,21 @@ class HostIndex:
         _check(load_library().gb_index_save(C.byref(self.view), str(path).encode()), "gb_index_save")
 
     @classmethod
-    def from_gbz(cls, path, k=29, w=11):
-        """gb_index_from_gbz: the flat index of a GBZ file (graphs that are chains of bubbles)."""
+    def from_gbz(cls, path, k=29, w=11, device=None):
+        """gb_index_from_gbz: the flat index of a GBZ file (graphs that are chains of bubbles).  device = a CUDA ordinal:
+        gb_index_from_gbz_device, the minimizers enumerated on that GPU (the same index)."""
         lib = load_library()
         h = C.c_void_p()
-        _check(lib.gb_index_from_gbz(str(path).encode(), k, w, C.byref(h)), "gb_index_from_gbz")
+        if device is None:
+            _check(lib.gb_index_from_gbz(str(path).encode(), k, w, C.byref(h)), "gb_index_from_gbz")
+        else:
+            _check(lib.gb_index_from_gbz_device(str(path).encode(), k, w, device, C.byref(h)), "gb_index_from_gbz_device")
         return cls.__new__(cls)._adopt(h, None, None, k, w)
 
     @classmethod
-    def from_gbwt(cls, node_seqs, n_paths, gbwt_words, rec_off, dist=None, k=29, w=11, hits=None):
-        """gb_index_build_from_gbwt: node sequences + a flat GBWT (gb_flat_index blob layout) instead of haplotype paths."""
+    def from_gbwt(cls, node_seqs, n_paths, gbwt_words, rec_off, dist=None, k=29, w=11, hits=None, device=None):
+        """gb_index_build_from_gbwt: node sequences + a flat GBWT (gb_flat_index blob layout) instead of haplotype paths.
+        device = a CUDA ordinal: gb_index_build_from_gbwt_device, the minimizers enumerated on that GPU (the same index)."""
         lib = load_library()
         n = len(node_seqs)
         node_off = np.zeros(n + 1, dtype=np.uint64)
@@ -347,10 +360,19 @@ class HostIndex:
         if hits is not None:
             hk, hp = (np.ascontiguousarray(a, dtype=np.uint64) for a in hits)
         h = C.c_void_p()
-        _check(lib.gb_index_build_from_gbwt(n, ptr(seq), ptr(node_off), n_paths, ptr(words), len(words), ptr(ro), dptr, k, w,
-                                            0 if hk is None else len(hk), None if hk is None else ptr(hk), None if hp is None else ptr(hp),
-                                            C.byref(h)), "gb_index_build_from_gbwt")
+        args = (n, ptr(seq), ptr(node_off), n_paths, ptr(words), len(words), ptr(ro), dptr, k, w,
+                0 if hk is None else len(hk), None if hk is None else ptr(hk), None if hp is None else ptr(hp))
+        if device is None:
+            _check(lib.gb_index_build_from_gbwt(*args, C.byref(h)), "gb_index_build_from_gbwt")
+        else:
+            _check(lib.gb_index_build_from_gbwt_device(*args, device, C.byref(h)), "gb_index_build_from_gbwt_device")
         return cls.__new__(cls)._adopt(h, list(node_seqs), None, k, w)
+
+    def timing(self) -> dict:
+        """gb_index_build_timing: host-clocked seconds of each build step and the minimizer step's counts."""
+        t = IndexTiming()
+        _check(load_library().gb_index_build_timing(self._h, C.byref(t)), "gb_index_build_timing")
+        return {name: getattr(t, name) for name, _ in IndexTiming._fields_}
 
     @classmethod
     def from_gbz_min(cls, gbz, min_path, zipcodes=None):

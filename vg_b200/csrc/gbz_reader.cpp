@@ -21,6 +21,7 @@
 // Only what this path needs is kept; anything the reader does not understand is GB_ERR_FORMAT, never a guess.
 #include "giraffe_b200.h"
 #include "entry_guard.h"
+#include "index_build.h"
 
 #include <algorithm>
 #include <cstdio>
@@ -181,9 +182,14 @@ static int count_zipcodes(const char* path, uint64_t& count) {
     return GB_OK;
 }
 
-static int index_from_gbz_impl(const char* path, uint32_t k, uint32_t w, gb_host_index** out, const MinFile* min = nullptr) {
+// device < 0: the whole build on the host; device >= 0: the minimizers are enumerated on that GPU (gb_index_from_gbz_device).
+static int index_from_gbz_impl(const char* path, uint32_t k, uint32_t w, gb_host_index** out, const MinFile* min = nullptr, int device = -1) {
     if (!path || !out) return GB_ERR_ARG;
     *out = nullptr;
+    if (device >= 0) {
+        if (k == 0 || k > 31 || w == 0) return GB_ERR_ARG;
+        if (const int rc = gb::device_ready(device)) return rc;
+    }
     FILE* f = fopen(path, "rb");
     if (!f) return fail("open");
     std::vector<uint8_t> bytes;
@@ -275,14 +281,24 @@ static int index_from_gbz_impl(const char* path, uint32_t k, uint32_t w, gb_host
     // tables, see gb_dist_payload: nested bubbles, multi-node alleles and adjacent variants are all fine), minimizers by window
     // enumeration over GBWT search states, or taken from the .min file ----
     if (node_seq.empty()) node_seq.push_back(0);
-    const int rc = gb_index_build_from_gbwt((uint32_t)n_ids, node_seq.data(), node_off.data(), (uint32_t)(sequences / 2), blob.data(), blob.size(), rec_off.data(),
-                                            nullptr, k, w, min ? min->keys.size() : 0, min ? min->keys.data() : nullptr, min ? min->pos.data() : nullptr, out);
+    const int rc = gb::guarded("gb_index_build_from_gbwt", [&] {
+        return gb::index_build_from_gbwt(device, (uint32_t)n_ids, node_seq.data(), node_off.data(), (uint32_t)(sequences / 2), blob.data(), blob.size(),
+                                         rec_off.data(), nullptr, k, w, min ? min->keys.size() : 0, min ? min->keys.data() : nullptr,
+                                         min ? min->pos.data() : nullptr, out);
+    });
     if (rc == GB_OK && !gb_index_has_distance_model(*out)) { gb_index_free(*out); *out = nullptr; return fail("graph outside the chain model (cycle, reversing haplotype or oversized site)"); }
     return rc;
 }
 
 extern "C" int gb_index_from_gbz(const char* path, uint32_t k, uint32_t w, gb_host_index** out) {
     return gb::guarded("gb_index_from_gbz", GB_ERR_FORMAT, [&] { return index_from_gbz_impl(path, k, w, out); }, [&] { if (out) *out = nullptr; });
+}
+
+extern "C" int gb_index_from_gbz_device(const char* path, uint32_t k, uint32_t w, int device_ordinal, gb_host_index** out) {
+    return gb::guarded("gb_index_from_gbz_device", GB_ERR_FORMAT, [&] {
+        if (device_ordinal < 0) { if (out) *out = nullptr; return GB_ERR_ARG; }
+        return index_from_gbz_impl(path, k, w, out, nullptr, device_ordinal);
+    }, [&] { if (out) *out = nullptr; });
 }
 
 extern "C" int gb_index_from_gbz_min(const char* gbz_path, const char* min_path, const char* zipcodes_path, gb_host_index** out) {

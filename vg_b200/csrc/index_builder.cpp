@@ -12,9 +12,11 @@
 
 #include "giraffe_b200.h"
 #include "entry_guard.h"
+#include "index_build.h"
 #include "minimizer_common.h"
 
 #include <algorithm>
+#include <chrono>
 #include <cstdlib>
 #include <array>
 #include <cstdio>
@@ -38,6 +40,7 @@ struct gb_host_index {
     std::vector<gb_slot_rec> slots;
     std::vector<uint16_t> site_dist;
     bool model_ok = true;            // the distance payload is valid (given by the caller or derived)
+    gb_index_timing timing{};        // how the build spent its time (gb_index_build_timing)
 };
 
 namespace {
@@ -277,7 +280,7 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
                             const gb_dist_payload* dist, uint32_t k, uint32_t w,
                             gb_host_index** out,
                             uint64_t n_ext_hits = 0, const uint64_t* ext_keys = nullptr, const uint64_t* ext_pos = nullptr,
-                            const std::vector<GbwtRecordIn>* records = nullptr) {
+                            const std::vector<GbwtRecordIn>* records = nullptr, int device = -1) {
     if (!node_seq || !node_off || !out || (!records && n_paths && (!path_nodes || !path_off))) return GB_ERR_ARG;
     if (records && records->size() != 2 * ((size_t)n_node_ids + 1)) return GB_ERR_ARG;
     const bool external = ext_keys != nullptr || ext_pos != nullptr;
@@ -288,6 +291,11 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
     if (n_node_ids >= 0x7ffffff0u || 2 * node_off[n_node_ids] + 64 > 0xffffffffull) return GB_ERR_FORMAT;
     auto* ix = new gb_host_index();
     ix->k = k; ix->w = w; ix->n_paths = n_paths;
+    auto clock = std::chrono::steady_clock::now();
+    auto lap = [&](double& seconds) {
+        const auto now = std::chrono::steady_clock::now();
+        seconds = std::chrono::duration<double>(now - clock).count(); clock = now;
+    };
     ix->n_nodes = 2 * (n_node_ids + 1);
     ix->nodes.assign(ix->n_nodes, gb_node_rec{0, 0, 0, 0});
 
@@ -306,6 +314,7 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
         for (uint64_t i = e; i > b; i--) ix->seq.push_back(comp(node_seq[i - 1]));
     }
     ix->seq.resize(ix->seq.size() + 64, 0);
+    lap(ix->timing.sequences_s);
 
     ix->dist.assign(n_node_ids + 1, gb_dist_payload{0, 0, 0, 0xFFFF, 0});
     if (dist) for (uint32_t id = 1; id <= n_node_ids; id++) ix->dist[id] = dist[id];
@@ -341,6 +350,7 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
             ix->slots.clear(); ix->site_dist.clear(); ix->model_ok = false;
         }
     }
+    lap(ix->timing.distance_s);
 
     // --- bidirectional GBWT ---
     std::vector<std::vector<uint32_t>> seqs(records ? 0 : 2 * (size_t)n_paths);
@@ -461,10 +471,13 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
         }
     }
     ix->gbwt.resize(ix->gbwt.size() + 64, 0);
+    lap(ix->timing.gbwt_s);
 
     // --- minimizer index over forward haplotypes ---
-    struct KP { uint64_t key; uint64_t pos; };
+    using KP = gb::KeyPos;
     std::vector<KP> kps;
+    gb::WindowCounts counts;
+    bool sorted = false;                              // kps is already sorted and unique (the device route)
     std::string hap; std::vector<uint32_t> base_node; std::vector<uint32_t> base_off;
     std::vector<gbmin::Minimizer> mins;
     if (external) {
@@ -492,15 +505,22 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
     // gbwtgraph @ e27bc43, absent): every haplotype-consistent window of k + w - 1 bases is visited ONCE, however many haplotypes
     // share it, by following GBWT search states from every start position — work ~ graph x local diversity.  The minimizers of a
     // sequence are the union of the minimizers of its windows, so both give the same table (tests/test_gbz.py builds both).
-    // Chosen by the haplotype count (more than 32: windows); GIRAFFE_B200_WINDOW_BUILDER=0|1 forces one.
+    // Chosen by the haplotype count (more than 32: windows); GIRAFFE_B200_WINDOW_BUILDER=0|1 forces one.  A device build
+    // (device >= 0, always from records) enumerates the windows on the GPU: only the sorted pair list comes from elsewhere.
     bool use_windows = n_paths > 32;
     if (const char* env = std::getenv("GIRAFFE_B200_WINDOW_BUILDER")) use_windows = std::atoi(env) != 0;
     if (records) use_windows = true;                   // there are no paths to scan
+    const uint32_t W = k + w - 1;
+    bool forward_only = true;                          // every haplotype stays on forward strands: forward starts cover every window
     if (use_windows && !external) {
-        const uint32_t W = k + w - 1;
-        bool forward_only = true;                      // every haplotype stays on forward strands: forward starts cover every window
         if (records) { for (uint32_t v = 2; v < ix->n_nodes && forward_only; v += 2) for (const auto& e : (*records)[v].edges) if (e.first & 1u) { forward_only = false; break; } }
         else for (uint32_t p = 0; p < n_paths && forward_only; p++) for (uint32_t v : seqs[2 * p]) if (v & 1u) { forward_only = false; break; }
+    }
+    if (use_windows && !external && device >= 0) {
+        const int rc = gb::window_pairs_device(device, ix->nodes, ix->seq, ix->gbwt, k, w, forward_only, kps, counts);
+        if (rc != GB_OK) { delete ix; return rc; }
+        sorted = true;
+    } else if (use_windows && !external) {
         // successors of a GBWT search state (node, [lo, hi]) in record order
         auto follow = [&](uint32_t v, int64_t lo, int64_t hi, std::vector<std::array<int64_t, 3>>& out) {
             out.clear();
@@ -533,6 +553,7 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
         auto process = [&](size_t len) {
             mins.clear();
             gbmin::minimizers((const uint8_t*)win.data(), len, k, w, mins, nullptr);
+            counts.continuations++; counts.raw_pairs += mins.size();
             for (const auto& m : mins) {
                 uint32_t v = wnode[m.offset], o = woff[m.offset];
                 if (m.is_reverse) { o = ix->nodes[v].len - 1 - o; v ^= 1u; }
@@ -541,6 +562,7 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
         };
         for (uint32_t v0 = 2; v0 < ix->n_nodes; v0++) {
             if (ix->nodes[v0].size == 0 || (forward_only && (v0 & 1u))) continue;
+            counts.start_nodes++;
             const size_t need = (size_t)ix->nodes[v0].len + W - 1;
             stack.clear();
             stack.push_back(Frame{v0, 0, (int64_t)ix->nodes[v0].size - 1, 0});
@@ -571,14 +593,20 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
         }
         mins.clear();
         gbmin::minimizers((const uint8_t*)hap.data(), hap.size(), k, w, mins, nullptr);
+        counts.raw_pairs += mins.size();
         for (const auto& m : mins) {
             uint32_t v = base_node[m.offset], o = base_off[m.offset];
             if (m.is_reverse) { o = ix->nodes[v].len - 1 - o; v ^= 1u; }
             kps.push_back(KP{m.key, ((uint64_t)v << 10) | o});
         }
     }
-    std::sort(kps.begin(), kps.end(), [](const KP& a, const KP& b) { return a.key != b.key ? a.key < b.key : a.pos < b.pos; });
-    kps.erase(std::unique(kps.begin(), kps.end(), [](const KP& a, const KP& b) { return a.key == b.key && a.pos == b.pos; }), kps.end());
+    if (!sorted) {
+        std::sort(kps.begin(), kps.end(), [](const KP& a, const KP& b) { return a.key != b.key ? a.key < b.key : a.pos < b.pos; });
+        kps.erase(std::unique(kps.begin(), kps.end(), [](const KP& a, const KP& b) { return a.key == b.key && a.pos == b.pos; }), kps.end());
+    }
+    lap(ix->timing.minimizers_s);
+    ix->timing.start_nodes = counts.start_nodes; ix->timing.continuations = counts.continuations;
+    ix->timing.raw_pairs = external ? n_ext_hits : counts.raw_pairs; ix->timing.unique_pairs = kps.size();
     if (kps.size() > 0xfffffff0ull) { delete ix; return GB_ERR_FORMAT; }          // hit_off / hit_cnt are 32-bit
     size_t nkeys = 0;
     for (size_t i = 0; i < kps.size(); i++) if (i == 0 || kps[i].key != kps[i - 1].key) nkeys++;
@@ -597,6 +625,7 @@ static int index_build_impl(uint32_t n_node_ids, const uint8_t* node_seq, const 
         ix->table[h] = gb_min_cell{kps[i].key, (uint32_t)i, (uint32_t)(j - i)};
         i = j;
     }
+    lap(ix->timing.table_s);
     *out = ix;
     return GB_OK;
 }
@@ -622,29 +651,57 @@ extern "C" int gb_index_build_with_hits(uint32_t n_node_ids, const uint8_t* node
 
 // The index from node sequences and a flat GBWT (the blob layout of gb_flat_index.gbwt) instead of haplotype paths: nothing here
 // walks a haplotype, so the work follows the size of the graph, not haplotypes x genome.
+int gb::index_build_from_gbwt(int device, uint32_t n_node_ids, const uint8_t* node_seq, const uint64_t* node_off, uint32_t n_paths,
+                              const uint32_t* gbwt_words, uint64_t n_words, const uint32_t* rec_off, const gb_dist_payload* dist,
+                              uint32_t k, uint32_t w, uint64_t n_hits, const uint64_t* keys, const uint64_t* positions, gb_host_index** out) {
+    if (!gbwt_words || !rec_off || !out || n_node_ids >= 0x7ffffff0u) return GB_ERR_ARG;
+    if (device >= 0) {
+        // the arguments index_build_impl refuses, before the device is touched
+        if (!node_seq || !node_off || k == 0 || k > 31 || w == 0) return GB_ERR_ARG;
+        if (const int rc = gb::device_ready(device)) return rc;
+    }
+    const size_t n_nodes = 2 * ((size_t)n_node_ids + 1);
+    std::vector<GbwtRecordIn> records(n_nodes);
+    for (size_t v = 2; v < n_nodes; v++) {
+        const uint64_t off = rec_off[v];
+        if (off == 0) continue;
+        if (off + 2 > n_words) return GB_ERR_FORMAT;
+        const uint64_t n_edges = gbwt_words[off], n_runs = gbwt_words[off + 1];
+        if (n_edges >= 1024 || off + 2 + 2 * n_edges + n_runs > n_words) return GB_ERR_FORMAT;
+        GbwtRecordIn& rc = records[v];
+        for (uint64_t e = 0; e < n_edges; e++) rc.edges.push_back({gbwt_words[off + 2 + 2 * e], gbwt_words[off + 3 + 2 * e]});
+        for (uint64_t r = 0; r < n_runs; r++) { const uint32_t wd = gbwt_words[off + 2 + 2 * n_edges + r]; rc.runs.push_back({wd & 1023u, (uint64_t)(wd >> 10)}); }
+    }
+    static const uint64_t none = 0;
+    const bool ext = keys || positions;
+    if (ext && n_hits == 0) { keys = keys ? keys : &none; positions = positions ? positions : &none; }
+    return index_build_impl(n_node_ids, node_seq, node_off, n_paths, nullptr, nullptr, dist, k, w, out, n_hits, keys, positions, &records, device);
+}
+
 extern "C" int gb_index_build_from_gbwt(uint32_t n_node_ids, const uint8_t* node_seq, const uint64_t* node_off, uint32_t n_paths,
                                         const uint32_t* gbwt_words, uint64_t n_words, const uint32_t* rec_off,
                                         const gb_dist_payload* dist, uint32_t k, uint32_t w,
                                         uint64_t n_hits, const uint64_t* keys, const uint64_t* positions, gb_host_index** out) {
     return gb::guarded("gb_index_build_from_gbwt", [&] {
-        if (!gbwt_words || !rec_off || !out || n_node_ids >= 0x7ffffff0u) return GB_ERR_ARG;
-        const size_t n_nodes = 2 * ((size_t)n_node_ids + 1);
-        std::vector<GbwtRecordIn> records(n_nodes);
-        for (size_t v = 2; v < n_nodes; v++) {
-            const uint64_t off = rec_off[v];
-            if (off == 0) continue;
-            if (off + 2 > n_words) return GB_ERR_FORMAT;
-            const uint64_t n_edges = gbwt_words[off], n_runs = gbwt_words[off + 1];
-            if (n_edges >= 1024 || off + 2 + 2 * n_edges + n_runs > n_words) return GB_ERR_FORMAT;
-            GbwtRecordIn& rc = records[v];
-            for (uint64_t e = 0; e < n_edges; e++) rc.edges.push_back({gbwt_words[off + 2 + 2 * e], gbwt_words[off + 3 + 2 * e]});
-            for (uint64_t r = 0; r < n_runs; r++) { const uint32_t wd = gbwt_words[off + 2 + 2 * n_edges + r]; rc.runs.push_back({wd & 1023u, (uint64_t)(wd >> 10)}); }
-        }
-        static const uint64_t none = 0;
-        const bool ext = keys || positions;
-        if (ext && n_hits == 0) { keys = keys ? keys : &none; positions = positions ? positions : &none; }
-        return index_build_impl(n_node_ids, node_seq, node_off, n_paths, nullptr, nullptr, dist, k, w, out, n_hits, keys, positions, &records);
+        return gb::index_build_from_gbwt(-1, n_node_ids, node_seq, node_off, n_paths, gbwt_words, n_words, rec_off, dist, k, w, n_hits, keys, positions, out);
     });
+}
+
+extern "C" int gb_index_build_from_gbwt_device(uint32_t n_node_ids, const uint8_t* node_seq, const uint64_t* node_off, uint32_t n_paths,
+                                               const uint32_t* gbwt_words, uint64_t n_words, const uint32_t* rec_off,
+                                               const gb_dist_payload* dist, uint32_t k, uint32_t w,
+                                               uint64_t n_hits, const uint64_t* keys, const uint64_t* positions,
+                                               int device_ordinal, gb_host_index** out) {
+    return gb::guarded("gb_index_build_from_gbwt_device", [&] {
+        if (device_ordinal < 0) return GB_ERR_ARG;
+        return gb::index_build_from_gbwt(device_ordinal, n_node_ids, node_seq, node_off, n_paths, gbwt_words, n_words, rec_off, dist, k, w, n_hits, keys, positions, out);
+    });
+}
+
+extern "C" int gb_index_build_timing(const gb_host_index* ix, gb_index_timing* out) {
+    if (!ix || !out) return GB_ERR_ARG;
+    *out = ix->timing;
+    return GB_OK;
 }
 
 extern "C" void gb_index_free(gb_host_index* ix) { delete ix; }

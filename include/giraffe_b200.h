@@ -111,7 +111,8 @@ typedef struct gb_min_cell {
 /* One located minimizer occurrence (24 B): packed position + payload
  * (vg: MinimizerIndex::get_value, minimizer_mapper.cpp:4458-4473).
  * pos = (v << 10) | offset, v = oriented node of the k-mer's first base in the k-mer's
- * own orientation (gbwtgraph Position::encode). */
+ * own orientation (gbwtgraph Position::encode).  payload = dist[v >> 1], the payload of the hit's node (the builders
+ * write it so; gb_index_load refuses a file where it differs). */
 typedef struct gb_hit {
     uint64_t pos;
     gb_dist_payload payload;
@@ -405,8 +406,13 @@ void gb_map_params_default(gb_map_params* p);
  * mapping j of read r in output order (minimizer_mapper.cpp:1087-1206; map_paired: pair j of the pair, :2505-2598) —
  * j = 0 the primary, which alone carries the MAPQ; j >= 1 secondaries (GB_ALN_SECONDARY), or GB_ALN_ABSENT when the
  * read has fewer mappings.  With max_multimaps = 1 (the default) that is one record per read.
- * Limits of the mapping entry points: reads up to 512 bp; node ids below 2^22 (the seeding kernels pack id and offset into
- * 32 bits; GB_ERR_CAPACITY for a larger index — the stage seams gb_extend_batch etc. are not affected).
+ * Limits of the mapping entry points: reads up to 512 bp.  Index limits, the same for every mapping entry point:
+ *   node ids below 2^31 - 1 (n_nodes = 2 * (max_id + 1) is a uint32_t; tested past 2^22 with more than 2^22 real nodes
+ *   and with ids shifted up to 2^24);
+ *   sequence below 2^31 - 32 bp: both orientations are addressed by the 32-bit gb_node_rec.seq_off;
+ *   chain coordinates: x_in + length <= 2^31 - 1 and (int32) x_out - length >= -2^31 for every node with a sequence
+ *   (a payload the builder derives always fits; GB_ERR_CAPACITY from the mapping entry points for one that does not);
+ *   memory: nodes (16 B per oriented node) and dist (16 B per id) are dense over the ids: 48 B of HBM per id, used or not.
  * mappings / edits are DENSE pools of the given capacities
  * (gb_alignment.mapping_off / edit_off index into them); the elements used are returned
  * through n_mappings_used / n_edits_used (may be NULL).  GB_ERR_CAPACITY if a pool is too

@@ -227,6 +227,14 @@ extern "C" int gb_device_create(const gb_flat_index* ix, int device_ordinal, gb_
         d->h_node_len.resize(ix->n_nodes);
         d->h_dist.assign(ix->dist, ix->dist + ix->n_nodes / 2);
         for (uint32_t v = 0; v < ix->n_nodes; v++) d->h_node_len[v] = ix->nodes[v].len;
+        // c_in = x_in + offset and c_out = x_out - (length - offset) are int32 in the seeding kernels.  A derived payload
+        // always fits (x_in + length is at most the graph's sequence, below 2^31 by the 32-bit seq_off); a hand-made one may not.
+        for (uint32_t id = 1; id < ix->n_nodes / 2; id++) {
+            const uint32_t len = ix->nodes[2 * id].len;
+            if (len == 0) continue;
+            const gb_dist_payload& p = ix->dist[id];
+            if ((uint64_t)p.x_in + len > (uint64_t)INT32_MAX || (int64_t)(int32_t)p.x_out - len < (int64_t)INT32_MIN) { d->chain_coords_fit = false; break; }
+        }
         d->ix.nodes = d->nodes.ptr; d->ix.seq = d->seq.ptr; d->ix.gbwt = d->gbwt.ptr; d->ix.dist = d->dist.ptr;
         d->ix.table = d->table.ptr; d->ix.hits = d->hits.ptr;
         d->ix.table_mask = ix->table_cells - 1; d->ix.n_nodes = ix->n_nodes; d->ix.k = ix->k; d->ix.w = ix->w;

@@ -131,6 +131,7 @@ struct gb_device {
     int n_sms = 0;
     std::vector<uint32_t> h_node_len;      // host copy of the node lengths (workspace sizing of the DP seams)
     std::vector<gb_dist_payload> h_dist;   // host copy of the distance payload (fragment-length training)
+    bool chain_coords_fit = true;          // every used node's chain coordinates fit the mapping kernels' int32 c_in / c_out
     // first-pass seeding table sizes (minimizers, clusters per read); GIRAFFE_B200_SEED_TABLES="Mc,Cc" overrides
     uint32_t seed_mc = 64, seed_cc = 16, seed_ns = 64;
     cudaStream_t stream = nullptr, own_stream = nullptr;

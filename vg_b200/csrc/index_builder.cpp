@@ -814,7 +814,9 @@ static int index_load_impl(const char* path, gb_host_index** out) {
         for (uint64_t e = 0; e < n_edges; e++) if (rec[2 + 2 * e] >= h.n_nodes) { delete ix; return GB_ERR_FORMAT; }
         for (uint64_t t = 0; t < n_runs; t++) if ((rec[2 + 2 * n_edges + t] & 1023u) >= n_edges) { delete ix; return GB_ERR_FORMAT; }
     }
-    for (const gb_hit& hit : ix->hits) if ((hit.pos >> 10) >= h.n_nodes) { delete ix; return GB_ERR_FORMAT; }
+    // a hit carries its node's distance payload (the seeding kernels take two seeds on one node to share x_in)
+    for (const gb_hit& hit : ix->hits)
+        if ((hit.pos >> 10) >= h.n_nodes || memcmp(&hit.payload, &ix->dist[hit.pos >> 11], sizeof(gb_dist_payload)) != 0) { delete ix; return GB_ERR_FORMAT; }
     // slot tables stay inside site_dist, and a node that claims a place in a site table really has one
     for (const gb_slot_rec& sr : ix->slots)
         if (sr.table_off != 0xFFFFFFFFu && (uint64_t)sr.table_off + (uint64_t)sr.n * sr.n > h.site_dist_len) { delete ix; return GB_ERR_FORMAT; }

@@ -465,8 +465,8 @@ int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const ui
                const uint64_t* d_run_base, uint32_t read_base, uint64_t* d_totals, uint32_t* d_overflow) {
     int rc;
     if (hp->max_multimaps == 0 || hp->max_multimaps > GB_MAX_MULTIMAPS) { g_last_error = "max_multimaps must be 1 .. GB_MAX_MULTIMAPS"; return GB_ERR_ARG; }
-    // the seeding kernels pack (node id << 10 | offset) into 32 bits (DevSeed.id_off): node ids stop at 2^22 - 1
-    if (d->ix.n_nodes > (1u << 23)) { g_last_error = "the mapping kernels address node ids below 2^22 (4 194 303); split the graph (the stage seams have no such limit)"; return GB_ERR_CAPACITY; }
+    // node ids are those of the 32-bit n_nodes (below 2^31 - 1); chain coordinates must fit the seeds' int32 c_in / c_out
+    if (!d->chain_coords_fit) { g_last_error = "the index's chain coordinates do not fit 32 bits (x_in + node length above 2^31 - 1, or x_out - node length below -2^31)"; return GB_ERR_CAPACITY; }
     const uint32_t K = hp->max_multimaps;            // records per read, rank-major: record j * n_reads + read
     if ((uint64_t)n_reads * K * std::max(hp->mapping_cap_per_read, hp->edit_cap_per_read) > 0xffffffffull) { g_last_error = "chunk too large for 32-bit record offsets (reads x max_multimaps x cap)"; return GB_ERR_ARG; }
     if ((rc = d->pad_maps.reserve((size_t)n_reads * K * hp->mapping_cap_per_read))) return rc;

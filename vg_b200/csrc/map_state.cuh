@@ -99,8 +99,10 @@ struct __align__(16) DevSeed {
     int32_t  c_out;           // x_out - (len - off_fwd): coordinate when the seed is the source
     int32_t  c_in;            // x_in + off_fwd:          coordinate when the seed is the target
     uint32_t slot;
-    uint32_t id_off;          // (node id << 10) | forward-strand offset
 };
+// A hit's payload is the distance payload of its node id (gb_hit), so two seeds on one node share x_in and their c_in
+// differ by their forward offsets: the seed needs no packed (id, offset) word, and node ids keep all 31 bits.
+static_assert(sizeof(DevSeed) == 32, "DevSeed must be 32 bytes");
 
 // One (read, cluster) work item for the extension kernel, in processing order.
 struct __align__(16) DevItem {

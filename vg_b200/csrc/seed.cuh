@@ -198,10 +198,10 @@ __device__ __forceinline__ bool any_bit_in_range(const uint32_t* words, uint32_t
 
 // unoriented minimum graph distance <= limit between two seeds (see gb_dist_payload)
 // Two different nodes of one site: distance through the site's table (either direction), INT_MAX when unreachable.
-// id_off = (node id << 10) | forward offset; c_in = x_in + offset, c_out = x_out - (length - offset).
-__device__ __noinline__ int32_t same_site_distance(const DevIndex& ix, uint32_t ido_a, int32_t c_in_a, int32_t c_out_a, uint32_t ido_b, int32_t c_in_b, int32_t c_out_b) {
+// c_in = x_in + offset, c_out = x_out - (length - offset), offsets on the forward strand.
+__device__ __noinline__ int32_t same_site_distance(const DevIndex& ix, uint32_t id_a, int32_t c_in_a, int32_t c_out_a, uint32_t id_b, int32_t c_in_b, int32_t c_out_b) {
     if (ix.n_slots == 0) return INT_MAX;
-    const uint4 pa = __ldg(reinterpret_cast<const uint4*>(ix.dist) + (ido_a >> 10)), pb = __ldg(reinterpret_cast<const uint4*>(ix.dist) + (ido_b >> 10));
+    const uint4 pa = __ldg(reinterpret_cast<const uint4*>(ix.dist) + id_a), pb = __ldg(reinterpret_cast<const uint4*>(ix.dist) + id_b);
     int64_t best = -1;
     int64_t t = site_distance(ix, pa, pb);                       // a -> b: rest of a + table + offset in b
     if (t >= 0) best = ((int64_t)(int32_t)pa.y - c_out_a) + t + ((int64_t)c_in_b - (int64_t)(int32_t)pb.x);
@@ -211,14 +211,14 @@ __device__ __noinline__ int32_t same_site_distance(const DevIndex& ix, uint32_t 
 }
 
 __device__ __forceinline__ bool seeds_within(const DevIndex& ix, const DevSeed& a, const DevSeed& b, int32_t limit) {
-    const uint32_t ida = a.id_off >> 10, idb = b.id_off >> 10;
+    const uint32_t ida = a.node >> 1, idb = b.node >> 1;
     if (ida == idb) {
-        const int32_t d = (int32_t)(b.id_off & 1023u) - (int32_t)(a.id_off & 1023u);
+        const int32_t d = b.c_in - a.c_in;                        // one node, one x_in: the forward offsets' difference
         return (d >= 0 ? d : -d) <= limit;
     }
     if (a.slot < b.slot) return (b.c_in - a.c_out) <= limit;
     if (b.slot < a.slot) return (a.c_in - b.c_out) <= limit;
-    return same_site_distance(ix, a.id_off, a.c_in, a.c_out, b.id_off, b.c_in, b.c_out) <= limit;
+    return same_site_distance(ix, ida, a.c_in, a.c_out, idb, b.c_in, b.c_out) <= limit;
 }
 
 // -----------------------------------------------------------------------------------------
@@ -615,7 +615,6 @@ __device__ __forceinline__ uint32_t seed_phase_a(const DevIndex& ix, const MapPa
             sd.c_in = (int32_t)p1.x + (int32_t)off_f;
             sd.c_out = (int32_t)p1.y - (int32_t)(nlen - off_f);
             sd.slot = p2.x;
-            sd.id_off = ((node >> 1) << 10) | off_f;
             seeds[idx] = sd;
         }
     }
@@ -638,8 +637,9 @@ __device__ __forceinline__ void propagate_labels(const DevIndex& ix, DevSeed* se
             uint32_t best = si.label;
             for (uint32_t j = 0; j < n; j++) {
                 if (j == i) continue;
-                const DevSeed sj = j < na ? seeds_a[j] : seeds_b[j - na];
-                if (sj.label < best && seeds_within(ix, si, sj, limit)) best = sj.label;
+                const DevSeed* pj = j < na ? seeds_a + j : seeds_b + (j - na);
+                const uint32_t lj = pj->label;
+                if (lj < best && seeds_within(ix, si, *pj, limit)) best = lj;
             }
             if (best != si.label) { pi->label = best; changed = true; }
         }
@@ -658,7 +658,7 @@ struct ClusterScratch {
     uint8_t* has_pair;     // [F]
     uint32_t F;
     // joint clustering of small seed sets in shared memory (whatever is left of the dead arrays)
-    uint4* seedbuf;        // [ns_cap]  (id_off, c_in, c_out, slot)
+    uint4* seedbuf;        // [ns_cap]  (node id, c_in, c_out, slot)
     uint8_t* lab_frag;     // [ns_cap]  fragment label (index in the concatenation of both reads)
     uint8_t* lab_read;     // [ns_cap]  read-cluster label (same index space)
     uint32_t ns_cap;       // <= 64
@@ -901,7 +901,7 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
 #pragma unroll 1
         for (uint32_t i = lane; i < n_all; i += 32) {
             const DevSeed sd = i < H0 ? seeds_of(0)[i] : seeds_of(1)[i - H0];
-            cs.seedbuf[i] = make_uint4(sd.id_off, (uint32_t)sd.c_in, (uint32_t)sd.c_out, sd.slot);
+            cs.seedbuf[i] = make_uint4(sd.node >> 1, (uint32_t)sd.c_in, (uint32_t)sd.c_out, sd.slot);
         }
         __syncwarp();
         bool has[2]; uint64_t adj_f[2] = {0, 0}, adj_r[2] = {0, 0};
@@ -923,7 +923,7 @@ __device__ __forceinline__ uint32_t cluster_phase_pe(const DevIndex& ix, const M
                 const uint4 c = cs.seedbuf[j];
                 if (row >= n_all || row == j) continue;
                 int32_t d;
-                if ((a.x >> 10) == (c.x >> 10)) { d = (int32_t)(c.x & 1023u) - (int32_t)(a.x & 1023u); d = d >= 0 ? d : -d; }
+                if (a.x == c.x) { d = (int32_t)c.y - (int32_t)a.y; d = d >= 0 ? d : -d; }
                 else if (a.w < c.w) d = (int32_t)c.y - (int32_t)a.z;
                 else if (c.w < a.w) d = (int32_t)a.y - (int32_t)c.z;
                 else { pend |= 1ull << j; continue; }

@@ -918,6 +918,98 @@ int gb_chain_candidates_batch(gb_device* dev, uint32_t n_problems, const uint32_
                               uint64_t max_graph_lookback_bases, gb_chain_candidate* candidates, uint64_t candidate_cap,
                               uint64_t* cand_off);
 
+/* ------------------------------------------------------------------------------------
+ * Surjection onto reference paths and SAM output (`vg giraffe -o SAM`, giraffe_main.cpp:2164-2215):
+ * SurjectingAlignmentEmitter (surjecting_alignment_emitter.cpp:28-60) calls Surjector::surject (surjector.cpp:223-630)
+ * for every alignment, then HTSAlignmentEmitter writes alignment_to_sam_internal (alignment.cpp:607-754).
+ * Giraffe's defaults only: no --prune-low-cplx, no supplementaries (SA), no left-align, no GR / NR / SS tags.
+ * Not built here: the realigning route of realigning_surject (surjector.cpp:3255-3560, an alignment that leaves the
+ * reference path: gb_surject_device defers such records to the caller rather than write anything vg would not), spliced
+ * surjection, BAM and CRAM, @RG / RG, --comments-as-tags, @SQ M5, @PG, and
+ * reference paths read from GBZ metadata.
+ * ---------------------------------------------------------------------------------- */
+typedef struct gb_ref_paths gb_ref_paths;
+
+/* Reference paths in the caller's order (the --ref-paths / sequence-dictionary order, and the order of the @SQ lines):
+ * path p is named names[name_off[p] .. name_off[p+1]) and walks the oriented nodes path_nodes[path_off[p] .. path_off[p+1])
+ * in GBWT encoding (v = 2 * id + is_reverse), as a vg shim reads them off its PathPositionHandleGraph.  The result is a
+ * dense per-node-id record (path, strand, base offset of the node on the path) and each path's length.
+ *   GB_ERR_ARG     NULL arrays or out, decreasing offsets
+ *   GB_ERR_FORMAT  a node the graph does not have (id past the index, or an id without sequence); a node that occurs more
+ *                  than once across all reference paths (LIMIT: every node is on at most one reference path, once, so a
+ *                  read's path has one place on the references); a path of 2^31 bases or more (SAM / BAM positions are
+ *                  32-bit); an empty path; a name that is empty or holds a byte outside '!'..'~'
+ * Freed with gb_ref_paths_free. */
+int gb_ref_paths_build(const gb_flat_index* ix, uint32_t n_paths, const uint8_t* names, const uint64_t* name_off,
+                       const uint32_t* path_nodes, const uint64_t* path_off, gb_ref_paths** out);
+void gb_ref_paths_free(gb_ref_paths* rp);
+/* The SAM header HTSAlignmentEmitter writes for these paths with giraffe's defaults: "@HD\tVN:1.5\tSO:unknown" and one
+ * "@SQ\tSN:<name>\tLN:<length>" per path in the caller's order, each line ending in '\n'.  No M5 and no @PG (vg adds them
+ * from data this library does not hold).  GB_ERR_CAPACITY when out_cap is too small (*out_used = bytes needed). */
+int gb_sam_header(const gb_ref_paths* rp, char* out, uint64_t out_cap, uint64_t* out_used);
+/* Copies the reference paths to the handle's HBM (8 B per node id plus the names); they replace earlier ones.  GB_ERR_ARG
+ * when rp was built for a graph with a different node count than the handle's. */
+int gb_device_set_ref_paths(gb_device* dev, const gb_ref_paths* rp);
+
+/* One surjected record (40 B): what HTSAlignmentEmitter writes for one Alignment.  The CIGAR is ops cigar[cigar_off ..
+ * cigar_off + n_cigar) of the cigar pool in BAM encoding, length << 4 | op (M 0, I 1, D 2, S 4). */
+typedef struct gb_sam_record {
+    uint32_t read_id;
+    uint16_t flag;                /* SAM FLAG                                                               */
+    uint8_t  mapq;                /* MAPQ carried over from the input record; 0 when unmapped               */
+    uint8_t  route;               /* GB_SURJ_*                                                              */
+    int32_t  ref;                 /* reference path index, -1 unmapped                                      */
+    int32_t  pos;                 /* 0-based leftmost reference base, -1 unmapped                           */
+    int32_t  score;               /* AS: score_contiguous_alignment of the surjected path (0 when unmapped) */
+    int32_t  mate_ref, mate_pos;  /* paired: the mate's ref / pos (-1 unmapped); unpaired: -1, -1           */
+    int32_t  tlen;                /* compute_template_lengths (hts_alignment_emitter.cpp:812); unpaired: 0  */
+    uint32_t cigar_off, n_cigar;
+} gb_sam_record;
+
+#define GB_SURJ_DIRECT    0u      /* one path chunk covers the whole read (surjector.cpp:3235-3253): copied over        */
+#define GB_SURJ_UNMAPPED  1u      /* unmapped input, or no node of the read's path is on a reference path              */
+#define GB_SURJ_REALIGN   2u      /* deferred: the read, or its mate, leaves the reference path and needs vg's realigning
+                                     route, which is not built here.  No SAM line is written for it; the caller surjects
+                                     these records (and, paired, their mates: both carry this route) with vg's Surjector */
+#define GB_SURJ_ABSENT    3u      /* GB_ALN_ABSENT input rank: no record (the SAM emitter skips it)                    */
+
+/* Surjector::surject for records already in HBM (gb_map_batch_device / gb_map_paired_job_device outputs, or any records
+ * copied there); every array is a DEVICE address.  Record x of d_aln gives d_out[x].  Per record, on the paths set by
+ * gb_device_set_ref_paths:
+ *   - the read's path is cut into chunks as extract_overlapping_paths does (surjector.cpp:4109): consecutive mappings
+ *     on consecutive steps of one path strand.  One chunk over all mappings is the direct route: the path is copied, POS is
+ *     its leftmost reference base, CIGAR is cigar_against_path (alignment.cpp:1339: M for matches and substitutions,
+ *     reversed on the reverse strand, end insertions as S, simplify_cigar), the score is score_contiguous_alignment
+ *     (alignment_scorer.cpp:159-245) with vg's default scores 1/4/6/1/5 whatever gb_set_scores set: vg's Surjector keeps
+ *     its own default aligner (surjector.cpp:45-57), MAPQ is carried over.
+ *   - no mapping on a reference path: unmapped (surjector.cpp:436-480); a read with several chunks, and its mate when
+ *     paired: GB_SURJ_REALIGN, deferred (ref / pos -1, no CIGAR, no SAM line; *n_realign counts them, may be NULL).
+ *   - flags: sam_flag / determine_flag (alignment.cpp:697-754, :2898): 0x10 reverse, 0x4 unmapped, 0x100 for GB_ALN_SECONDARY.
+ * Paired records (GB_ALN_PAIRED) must come as the mappers lay them out: the mate of record x is record x ^ 1 (read_id ^ 1).
+ * They get 0x1, 0x40 / 0x80 (even / odd read), the mate's ref / pos, 0x8 / 0x20 from the mate, TLEN from
+ * compute_template_lengths, and 0x2 when both lie on one path facing each other and |TLEN| <= tlen_max (tlen_max 0: no
+ * limit; giraffe passes mean + 6 stdev of a finalized fragment distribution, giraffe_main.cpp:2334-2339).
+ *   GB_ERR_ARG       no reference paths on the handle, NULL arrays, a record gb_emit_gaf_device would refuse, a paired
+ *                    record whose mate is not at x ^ 1 (decided on the device; nothing is written)
+ *   GB_ERR_CAPACITY  cigar_cap is too small: *cigar_used is the pool size needed, nothing is written; also when the pool
+ *                    would pass 2^32 ops (cigar_off is 32-bit: split the batch)
+ * On success *cigar_used is the extent of the cigar pool used (a record's region is sized by its raw op count, so the
+ * pool may hold gaps).  The call synchronises once, for the pool size; the fill is left enqueued on the handle's stream. */
+int gb_surject_device(gb_device* dev, uint32_t n, const gb_alignment* d_aln, const gb_mapping* d_mappings, uint64_t mapping_pool_len,
+                      const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint64_t* d_read_off, int64_t tlen_max,
+                      gb_sam_record* d_out, uint32_t* d_cigar, uint64_t cigar_cap, uint64_t* cigar_used, uint32_t* n_realign);
+
+/* SAM alignment lines of surjected records, formatted on the GPU (alignment_to_sam_internal, alignment.cpp:607-695): QNAME
+ * (names, or read<i> when d_names is NULL; paired records lose a trailing [/_][12]; '*' when empty), FLAG, RNAME, 1-based
+ * POS, MAPQ, CIGAR, RNEXT ('=' on the same path, '*' without a mate location), PNEXT, TLEN, SEQ and QUAL reverse-complemented
+ * / reversed on the reverse strand (QUAL '*' when d_quals is NULL), then AS:i.  An unmapped paired record takes its mate's
+ * RNAME and POS (SAMv1 §2.4.1).  GB_SURJ_ABSENT and GB_SURJ_REALIGN records are skipped.  The header is gb_sam_header's.  The contract of
+ * gb_emit_gaf_device: GB_ERR_ARG for a record outside its read, cigar pool or paths (decided on the device), GB_ERR_CAPACITY
+ * with *out_used = bytes needed, one synchronisation, the fill left enqueued. */
+int gb_emit_sam_device(gb_device* dev, uint32_t n, const gb_sam_record* d_rec, const uint32_t* d_cigar, uint64_t cigar_len,
+                       uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals, const uint64_t* d_read_off,
+                       const uint8_t* d_names, const uint64_t* d_name_off, char* d_out, uint64_t out_cap, uint64_t* out_used);
+
 /* Kernel-only timing of the last gb_*_batch call on this handle, milliseconds
  * (CUDA events on the handle's stream around the kernels, copies excluded). */
 float gb_last_kernel_ms(const gb_device* dev);

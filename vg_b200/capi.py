@@ -192,6 +192,12 @@ def load_library() -> C.CDLL:
         "gb_emit_gam": (st, [fix, *emit]),
         "gb_emit_gaf_device": (st, [vp, *emit]),
         "gb_emit_gam_device": (st, [vp, *emit]),
+        "gb_ref_paths_build": (st, [fix, u32, vp, vp, vp, vp, C.POINTER(vp)]),
+        "gb_ref_paths_free": (None, [vp]),
+        "gb_sam_header": (st, [vp, vp, u64, C.POINTER(u64)]),
+        "gb_device_set_ref_paths": (st, [vp, vp]),
+        "gb_surject_device": (st, [vp, u32, vp, vp, u64, vp, u64, u32, vp, C.c_int64, vp, vp, u64, C.POINTER(u64), C.POINTER(u32)]),
+        "gb_emit_sam_device": (st, [vp, u32, vp, vp, u64, u32, vp, vp, vp, vp, vp, vp, u64, C.POINTER(u64)]),
         "gb_debug_seed_stage": (st, [vp, C.POINTER(MapParams), C.c_int, u32, vp, vp, vp, vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, u64]),
         "gb_device_pool_overflow": (st, [vp, C.POINTER(C.c_int)]),
         "gb_kernel_times": (st, [vp, u32, vp, vp, vp]),
@@ -485,6 +491,53 @@ def stage_buffers(n, per_read=(160, 1024, 64, 64, 1024)):
     """Output arrays of gb_debug_seed_stage / the oracle's twin for n reads."""
     return (np.zeros(n, dtype=stage_read_dt), np.zeros(n * per_read[0] + 16, dtype=stage_minimizer_dt), np.zeros(n * per_read[1] + 16, dtype=stage_seed_dt),
             np.zeros(n * per_read[2] + 16, dtype=stage_cluster_dt), np.zeros(n * per_read[3] + 16, dtype=stage_item_dt), np.zeros(n * per_read[4] + 16, dtype=seed_dt))
+
+
+sam_record_dt = np.dtype([("read_id", "<u4"), ("flag", "<u2"), ("mapq", "u1"), ("route", "u1"), ("ref", "<i4"), ("pos", "<i4"),
+                          ("score", "<i4"), ("mate_ref", "<i4"), ("mate_pos", "<i4"), ("tlen", "<i4"), ("cigar_off", "<u4"),
+                          ("n_cigar", "<u4")])
+SURJ_DIRECT, SURJ_UNMAPPED, SURJ_REALIGN, SURJ_ABSENT = 0, 1, 2, 3
+
+
+class RefPaths:
+    """Owns a gb_ref_paths: reference paths (name, oriented nodes in GBWT encoding) in @SQ order, checked against the graph
+    of flat_index (a FlatIndex view)."""
+
+    def __init__(self, flat_index, paths):
+        names = [n.encode() for n, _ in paths]
+        name_off = np.zeros(len(paths) + 1, dtype=np.uint64)
+        name_off[1:] = np.cumsum([len(n) for n in names])
+        nodes = np.asarray([v for _, p in paths for v in p] + [0], dtype=np.uint32)
+        path_off = np.zeros(len(paths) + 1, dtype=np.uint64)
+        path_off[1:] = np.cumsum([len(p) for _, p in paths])
+        nb = np.frombuffer(b"".join(names) + b"\0", dtype=np.uint8).copy()
+        h = C.c_void_p()
+        _check(load_library().gb_ref_paths_build(C.byref(flat_index), len(paths), ptr(nb), ptr(name_off), ptr(nodes), ptr(path_off),
+                                                 C.byref(h)), "gb_ref_paths_build")
+        self._h = h
+
+    @property
+    def handle(self):
+        return self._h
+
+    def sam_header(self) -> str:
+        lib, used = load_library(), C.c_uint64()
+        rc = lib.gb_sam_header(self._h, None, 0, C.byref(used))
+        assert rc == GB_ERR_CAPACITY or (rc == GB_OK and used.value == 0)
+        buf = C.create_string_buffer(used.value)
+        _check(lib.gb_sam_header(self._h, buf, used.value, C.byref(used)), "gb_sam_header")
+        return buf.raw[: used.value].decode()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            load_library().gb_ref_paths_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class FragmentDistribution:
@@ -854,6 +907,50 @@ class Device:
                          vp(names), vp(name_off), vp(o), o.numel(), C.byref(used)),
             out, lambda: torch.empty(max(1, used.value), dtype=torch.uint8, device=reads.device))
         _check(rc, "gb_emit_" + kind + "_device")
+        _check(lib.gb_device_synchronize(self._h), "gb_device_synchronize")
+        return out[: used.value]
+
+    def set_ref_paths(self, ref_paths: "RefPaths"):
+        _check(load_library().gb_device_set_ref_paths(self._h, ref_paths.handle), "gb_device_set_ref_paths")
+
+    def surject_device(self, aln, maps, edits, read_off, tlen_max=0, cigar=None):
+        """gb_surject_device over CUDA tensors (aln = 32-byte records, maps = 8-byte mappings, edits = 32-bit words, read_off =
+        int64 n_reads + 1): (records as a uint8 CUDA tensor of 40-byte gb_sam_record, the cigar pool as an int32 CUDA tensor,
+        the number of records deferred to the realigning route).  The cigar pool is `cigar` when large enough, otherwise a
+        new tensor of the size the first call reported."""
+        import torch
+        lib = load_library()
+        vp = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+        n, n_maps, n_edits = aln.numel() * aln.element_size() // 32, maps.numel() * maps.element_size() // 8, edits.numel() * edits.element_size() // 4
+        torch.cuda.current_stream(read_off.device).synchronize()
+        out = torch.empty(max(1, n) * 40, dtype=torch.uint8, device=read_off.device)
+        if cigar is None:
+            cigar = torch.empty(1, dtype=torch.int32, device=read_off.device)
+        used, n_realign = C.c_uint64(), C.c_uint32()
+        rc, cigar = _retry_on_capacity(
+            lambda c: lib.gb_surject_device(self._h, n, vp(aln), vp(maps), n_maps, vp(edits), n_edits, read_off.numel() - 1, vp(read_off),
+                                            int(tlen_max), vp(out), vp(c), c.numel(), C.byref(used), C.byref(n_realign)),
+            cigar, lambda: torch.empty(max(1, used.value), dtype=torch.int32, device=read_off.device))
+        _check(rc, "gb_surject_device")
+        _check(lib.gb_device_synchronize(self._h), "gb_device_synchronize")
+        return out[: n * 40], cigar, n_realign.value
+
+    def emit_sam_device(self, rec, cigar, reads, read_off, quals=None, names=None, name_off=None, out=None):
+        """gb_emit_sam_device over CUDA tensors (rec = 40-byte gb_sam_record bytes, cigar = the pool): the SAM lines as a uint8
+        CUDA tensor, complete when this returns."""
+        import torch
+        lib = load_library()
+        vp = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+        torch.cuda.current_stream(reads.device).synchronize()
+        if out is None:
+            out = torch.empty(1, dtype=torch.uint8, device=reads.device)
+        used = C.c_uint64()
+        rc, out = _retry_on_capacity(
+            lambda o: lib.gb_emit_sam_device(self._h, rec.numel() * rec.element_size() // 40, vp(rec), vp(cigar), cigar.numel(),
+                                             read_off.numel() - 1, vp(reads), vp(quals), vp(read_off), vp(names), vp(name_off),
+                                             vp(o), o.numel(), C.byref(used)),
+            out, lambda: torch.empty(max(1, used.value), dtype=torch.uint8, device=reads.device))
+        _check(rc, "gb_emit_sam_device")
         _check(lib.gb_device_synchronize(self._h), "gb_device_synchronize")
         return out[: used.value]
 

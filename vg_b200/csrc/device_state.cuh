@@ -227,4 +227,10 @@ struct gb_device {
         gb::DevBuf<int64_t> out;
     } pj;
     uint32_t pj_windows = 0; double pj_training_ms = 0.0;      // training windows of the last such call and their host-clocked time
+    // gb_device_set_ref_paths: per node id {path << 1 | the path walks the node reversed (0xFFFFFFFF: on no path), base offset
+    // of the node on the path}, and the path names addressed by ref_name_off[n_ref_paths + 1]
+    bool ref_ready = false; uint32_t n_ref_paths = 0;
+    gb::DevBuf<uint32_t> ref_node;
+    gb::DevBuf<uint8_t> ref_names; gb::DevBuf<uint64_t> ref_name_off;
+    gb::DevBuf<uint8_t> surj_ws;           // gb_surject_device: validation flag, per-record op counts, offsets, scan temporaries
 };

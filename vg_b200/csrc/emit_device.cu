@@ -1,6 +1,7 @@
-// emit_device.cu — gb_emit_gaf_device / gb_emit_gam_device: GAF lines and GAM messages formatted on the GPU from records
-// that are already in HBM.  The format and the record check are emit_format.h's, the code gb_emit_gaf / gb_emit_gam run on
-// the host, so the bytes are those the host emitters write for the same records.  This file is the driver.
+// emit_device.cu — gb_emit_gaf_device / gb_emit_gam_device / gb_emit_sam_device: GAF lines, GAM messages and SAM lines
+// formatted on the GPU from records that are already in HBM.  The GAF / GAM format and record check are emit_format.h's, the
+// code gb_emit_gaf / gb_emit_gam run on the host, so the bytes are those the host emitters write for the same records; the
+// SAM line is sam_format.h's.  This file is the driver, one for the three formats.
 //
 // Count / scan / fill, one thread per record:
 //   validate   every record with record_valid and every name offset with name_valid, one flag for the whole batch
@@ -12,6 +13,7 @@
 #include "giraffe_b200.h"
 #include "device_state.cuh"
 #include "emit_format.h"
+#include "sam_format.h"
 
 #include <cub/cub.cuh>
 
@@ -22,34 +24,55 @@ namespace {
 
 constexpr uint32_t EMIT_BLOCK = 128;
 
+// ---- formats --------------------------------------------------------------------------------------------------------
+// What the driver asks of a format: n records, n_checks items to validate, whether record x is written, and its bytes
+// over a sink.  FRAMED formats (GAM) add vg::io's group framing around each record's bytes.
+struct GafFormat {
+    static constexpr bool FRAMED = false;
+    EmitArgs A;
+    __host__ __device__ uint32_t n() const { return A.n; }
+    __host__ __device__ uint32_t n_checks() const { return A.n > A.n_reads ? A.n : A.n_reads; }
+    __device__ bool valid(uint32_t i) const { return (i >= A.n_reads || name_valid(A, i)) && (i >= A.n || record_valid(A, A.aln[i])); }
+    __device__ bool present(uint32_t x) const { return !(A.aln[x].flags & GB_ALN_ABSENT); }
+    template <class S> __device__ void body(S& s, uint32_t x) const { gaf_record(s, A, A.aln[x]); }
+};
+struct GamFormat : GafFormat {
+    static constexpr bool FRAMED = true;
+    template <class S> __device__ void body(S& s, uint32_t x) const { gam_message(s, A, A.aln[x]); }
+};
+struct SamFormat {
+    static constexpr bool FRAMED = false;
+    SamArgs A;
+    __host__ __device__ uint32_t n() const { return A.n; }
+    __host__ __device__ uint32_t n_checks() const { return A.n > A.n_reads ? A.n : A.n_reads; }
+    __device__ bool valid(uint32_t i) const { return (i >= A.n_reads || sam_name_valid(A, i)) && (i >= A.n || sam_record_valid(A, A.rec[i])); }
+    __device__ bool present(uint32_t x) const { return sam_present(A.rec[x]); }
+    template <class S> __device__ void body(S& s, uint32_t x) const { sam_line(s, A, A.rec[x]); }
+};
+
 // ---- kernels --------------------------------------------------------------------------------------------------------
-__global__ void emit_validate_kernel(EmitArgs A, uint32_t* bad) {
-    const uint32_t total = max(A.n, A.n_reads);
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        bool ok = true;
-        if (i < A.n_reads && !name_valid(A, i)) ok = false;
-        if (ok && i < A.n) ok = record_valid(A, A.aln[i]);
-        if (!ok) *bad = 1u;
-    }
+template <class F>
+__global__ void emit_validate_kernel(F f, uint32_t* bad) {
+    const uint32_t total = f.n_checks();
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x)
+        if (!f.valid(i)) *bad = 1u;
 }
 
-// bytes[x] = the record's line (GAF) or message (GAM), 0 for an absent rank; present[x] (GAM) = 1 for a written record.
-// Nothing is formatted when the batch was refused: the records may point anywhere.
-template <bool GAM>
-__global__ void emit_size_kernel(EmitArgs A, const uint32_t* bad, uint64_t* bytes, uint32_t* present) {
+// bytes[x] = the record's line (GAF, SAM) or message (GAM), 0 for a record that is not written; present[x] (GAM) = 1 for a
+// written record.  Nothing is formatted when the batch was refused: the records may point anywhere.
+template <class F>
+__global__ void emit_size_kernel(F f, const uint32_t* bad, uint64_t* bytes, uint32_t* present) {
     const bool refused = *bad != 0;
-    for (uint32_t x = blockIdx.x * blockDim.x + threadIdx.x; x <= A.n; x += gridDim.x * blockDim.x) {
+    const uint32_t n = f.n();
+    for (uint32_t x = blockIdx.x * blockDim.x + threadIdx.x; x <= n; x += gridDim.x * blockDim.x) {
         uint64_t sz = 0; uint32_t pr = 0;
-        if (x < A.n && !refused) {
-            const gb_alignment a = A.aln[x];
-            if (!(a.flags & GB_ALN_ABSENT)) {
-                Count c;
-                if (GAM) gam_message(c, A, a); else gaf_record(c, A, a);
-                sz = c.n; pr = 1;
-            }
+        if (x < n && !refused && f.present(x)) {
+            Count c;
+            f.body(c, x);
+            sz = c.n; pr = 1;
         }
         bytes[x] = sz;
-        if (GAM) present[x] = pr;
+        if (F::FRAMED) present[x] = pr;
     }
 }
 
@@ -67,34 +90,28 @@ __global__ void gam_frame_kernel(uint32_t n, const uint64_t* msg, const uint32_t
     }
 }
 
-template <bool GAM>
-__global__ void emit_fill_kernel(EmitArgs A, const uint64_t* msg, const uint32_t* pidx, const uint64_t* off, char* out) {
-    for (uint32_t x = blockIdx.x * blockDim.x + threadIdx.x; x < A.n; x += gridDim.x * blockDim.x) {
-        const gb_alignment a = A.aln[x];
-        if (a.flags & GB_ALN_ABSENT) continue;
+template <class F>
+__global__ void emit_fill_kernel(F f, const uint64_t* msg, const uint32_t* pidx, const uint64_t* off, char* out) {
+    const uint32_t n = f.n();
+    for (uint32_t x = blockIdx.x * blockDim.x + threadIdx.x; x < n; x += gridDim.x * blockDim.x) {
+        if (!f.present(x)) continue;
         Write w{out + off[x]};
-        if (GAM) {
+        if (F::FRAMED) {
             const uint32_t p = pidx[x];
-            if (p % GAM_GROUP == 0) gam_header(w, min(GAM_GROUP, pidx[A.n] - p));
+            if (p % GAM_GROUP == 0) gam_header(w, min(GAM_GROUP, pidx[n] - p));
             varint(w, msg[x]);
-            gam_message(w, A, a);
-        } else {
-            gaf_record(w, A, a);
         }
+        f.body(w, x);
     }
 }
 
-template <bool GAM>
-int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_mapping* d_mappings, uint64_t mapping_pool_len,
-                const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
-                const uint64_t* d_read_off, const uint8_t* d_names, const uint64_t* d_name_off, char* d_out, uint64_t out_cap, uint64_t* out_used) {
-    if (!d || !d_aln || !d_reads || !d_read_off || !d_out || !out_used) return GB_ERR_ARG;
+// The driver: validate, size, scan, one wait for the total, fill.  `who` names the entry point in gb_last_error().
+template <class F>
+int emit_run(gb_device* d, const F& f, char* d_out, uint64_t out_cap, uint64_t* out_used, const char* who) {
+    const uint32_t n = f.n();
     if (n == 0xffffffffu) return GB_ERR_ARG;                 // the scans run over n + 1 entries
     GB_CUDA(cudaSetDevice(d->device));
-    EmitArgs A;
-    A.n = n; A.aln = d_aln; A.maps = d_mappings; A.map_len = mapping_pool_len; A.edits = d_edits; A.edit_len = edit_pool_len;
-    A.n_reads = n_reads; A.reads = d_reads; A.quals = d_quals; A.read_off = d_read_off; A.names = d_names; A.name_off = d_name_off;
-    A.nodes = d->ix.nodes; A.seq = d->ix.seq; A.n_nodes = d->ix.n_nodes;
+    constexpr bool GAM = F::FRAMED;
 
     // workspace: status {refused, total bytes}, bytes[n + 1], framed[n + 1] (GAM), off[n + 1], present / pidx[n + 1] (GAM), scan temp
     const size_t m = (size_t)n + 1;
@@ -112,10 +129,10 @@ int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_ma
     if (rc) return rc;
 
     const uint32_t grid = (uint32_t)std::min<uint64_t>((m + EMIT_BLOCK - 1) / EMIT_BLOCK, (uint64_t)d->n_sms * 64);
-    const uint32_t vgrid = (uint32_t)std::min<uint64_t>(((uint64_t)std::max(n, n_reads) + EMIT_BLOCK) / EMIT_BLOCK, (uint64_t)d->n_sms * 64);
+    const uint32_t vgrid = (uint32_t)std::min<uint64_t>(((uint64_t)f.n_checks() + EMIT_BLOCK) / EMIT_BLOCK, (uint64_t)d->n_sms * 64);
     GB_CUDA(cudaMemsetAsync(status, 0, 2 * sizeof(uint64_t), d->stream));
-    emit_validate_kernel<<<vgrid, EMIT_BLOCK, 0, d->stream>>>(A, (uint32_t*)status);
-    emit_size_kernel<GAM><<<grid, EMIT_BLOCK, 0, d->stream>>>(A, (const uint32_t*)status, bytes, present);
+    emit_validate_kernel<<<vgrid, EMIT_BLOCK, 0, d->stream>>>(f, (uint32_t*)status);
+    emit_size_kernel<<<grid, EMIT_BLOCK, 0, d->stream>>>(f, (const uint32_t*)status, bytes, present);
     d->launches += 2;
     GB_CUDA(cudaGetLastError());
     if (GAM) {
@@ -130,17 +147,41 @@ int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_ma
     uint64_t h_status[2];
     GB_CUDA(cudaMemcpyAsync(h_status, status, sizeof h_status, cudaMemcpyDeviceToHost, d->stream));
     GB_CUDA(cudaStreamSynchronize(d->stream));              // the one wait: the total decides whether the fill runs
-    if (h_status[0] & 0xffffffffull) { g_last_error = GAM ? "gb_emit_gam_device: a record points outside its read, pools or the graph"
-                                                          : "gb_emit_gaf_device: a record points outside its read, pools or the graph"; return GB_ERR_ARG; }
+    if (h_status[0] & 0xffffffffull) { set_last_error(who, ": a record points outside its read, pools or the graph"); return GB_ERR_ARG; }
     const uint64_t total = h_status[1];
     *out_used = total;
-    if (total > out_cap) { g_last_error = "gb_emit_*_device: output capacity too small (*out_used holds the bytes needed)"; return GB_ERR_CAPACITY; }
+    if (total > out_cap) { set_last_error(who, ": output capacity too small (*out_used holds the bytes needed)"); return GB_ERR_CAPACITY; }
     if (n) {
-        emit_fill_kernel<GAM><<<grid, EMIT_BLOCK, 0, d->stream>>>(A, bytes, pidx, off, d_out);
+        emit_fill_kernel<<<grid, EMIT_BLOCK, 0, d->stream>>>(f, bytes, pidx, off, d_out);
         d->launches++;
         GB_CUDA(cudaGetLastError());
     }
     return GB_OK;
+}
+
+template <bool GAM>
+int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_mapping* d_mappings, uint64_t mapping_pool_len,
+                const uint32_t* d_edits, uint64_t edit_pool_len, uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals,
+                const uint64_t* d_read_off, const uint8_t* d_names, const uint64_t* d_name_off, char* d_out, uint64_t out_cap, uint64_t* out_used) {
+    if (!d || !d_aln || !d_reads || !d_read_off || !d_out || !out_used) return GB_ERR_ARG;
+    EmitArgs A;
+    A.n = n; A.aln = d_aln; A.maps = d_mappings; A.map_len = mapping_pool_len; A.edits = d_edits; A.edit_len = edit_pool_len;
+    A.n_reads = n_reads; A.reads = d_reads; A.quals = d_quals; A.read_off = d_read_off; A.names = d_names; A.name_off = d_name_off;
+    A.nodes = d->ix.nodes; A.seq = d->ix.seq; A.n_nodes = d->ix.n_nodes;
+    if (GAM) return emit_run(d, GamFormat{A}, d_out, out_cap, out_used, "gb_emit_gam_device");
+    return emit_run(d, GafFormat{A}, d_out, out_cap, out_used, "gb_emit_gaf_device");
+}
+
+int emit_sam_device(gb_device* d, uint32_t n, const gb_sam_record* d_rec, const uint32_t* d_cigar, uint64_t cigar_len,
+                    uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals, const uint64_t* d_read_off,
+                    const uint8_t* d_names, const uint64_t* d_name_off, char* d_out, uint64_t out_cap, uint64_t* out_used) {
+    if (!d || !d_rec || !d_reads || !d_read_off || !d_out || !out_used) return GB_ERR_ARG;
+    if (!d->ref_ready) { g_last_error = "gb_emit_sam_device: no reference paths on the handle (gb_device_set_ref_paths)"; return GB_ERR_ARG; }
+    SamArgs A;
+    A.n = n; A.rec = d_rec; A.cigar = d_cigar; A.cigar_len = cigar_len;
+    A.n_reads = n_reads; A.reads = d_reads; A.quals = d_quals; A.read_off = d_read_off; A.names = d_names; A.name_off = d_name_off;
+    A.n_paths = d->n_ref_paths; A.path_names = d->ref_names.ptr; A.path_name_off = d->ref_name_off.ptr;
+    return emit_run(d, SamFormat{A}, d_out, out_cap, out_used, "gb_emit_sam_device");
 }
 
 } // namespace
@@ -156,3 +197,10 @@ int emit_device(gb_device* d, uint32_t n, const gb_alignment* d_aln, const gb_ma
     }
 GB_EMIT_DEVICE_ENTRY(gb_emit_gaf_device, false)
 GB_EMIT_DEVICE_ENTRY(gb_emit_gam_device, true)
+
+extern "C" int gb_emit_sam_device(gb_device* dev, uint32_t n, const gb_sam_record* d_rec, const uint32_t* d_cigar, uint64_t cigar_len,
+                                  uint32_t n_reads, const uint8_t* d_reads, const uint8_t* d_quals, const uint64_t* d_read_off,
+                                  const uint8_t* d_names, const uint64_t* d_name_off, char* d_out, uint64_t out_cap, uint64_t* out_used) {
+    return gb::guarded("gb_emit_sam_device", [&] { return gb::emit_sam_device(dev, n, d_rec, d_cigar, cigar_len, n_reads, d_reads, d_quals,
+                                                                              d_read_off, d_names, d_name_off, d_out, out_cap, out_used); });
+}

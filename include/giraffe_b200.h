@@ -461,14 +461,17 @@ uint64_t gb_fragment_sample_size(const gb_fragment_distribution* f);
 /* The paired job as `vg giraffe` runs it without --fragment-mean/--fragment-stdev
  * (giraffe_main.cpp:2246-2400): while `f` is not finalized, pairs are taken in input order through
  * MinimizerMapper::map_paired(aln1, aln2, ambiguous_pair_buffer) (minimizer_mapper.cpp:1303-1395) —
- * both ends mapped single-ended on the GPU (training_window pairs per gb_map_batch call; pairs of a
- * window behind the finalizing pair are not consumed), pairs whose ends are both MAPQ 60 with score >=
+ * both ends mapped single-ended on the GPU (windows of training_window pairs, at most half the map chunk,
+ * each uploaded and trained by the same step as gb_map_paired_job_device; pairs of a window behind the
+ * finalizing pair are not consumed), pairs whose ends are both MAPQ 60 with score >=
  * 0.85 * match * length and whose distance is below max_fragment_length register it and keep their
  * single-ended records, every other pair is buffered; once finalized (or, at the end of the input,
  * finalized by force as giraffe_main.cpp:2283-2296 does) all remaining and all buffered pairs go through
  * gb_map_paired_batch with the estimated mean / stdev (p->fragment_mean / p->fragment_stdev are
  * ignored; `f` carries the distribution across calls).  Outputs as gb_map_paired_batch;
- * pair_route[n_reads / 2] receives GB_PAIR_* (may be NULL).  training_window 0 selects 2048. */
+ * pair_route[n_reads / 2] receives GB_PAIR_* (may be NULL).  training_window 0 selects 2048.  Refused with
+ * GB_ERR_ARG: a NULL p or f, a NULL required array when n_reads > 0, an odd n_reads, max_multimaps != 1.
+ * Workspace on the handle: gb_map_paired_job_device's for one training window, plus its reads and qualities. */
 int gb_map_paired_job(gb_device* dev, const gb_map_params* p, gb_fragment_distribution* f, uint32_t training_window,
                       uint32_t n_reads, const uint8_t* reads, const uint8_t* quals, const uint64_t* read_off,
                       gb_alignment* aln, gb_mapping* mappings, uint64_t mapping_pool_cap, uint32_t* edits, uint64_t edit_pool_cap,

@@ -1,8 +1,8 @@
 """gb_map_paired_job_device: the paired job (fragment-length training, map_paired with the learned distribution, the
-ambiguous-pair buffer) on reads already in HBM.  The host job gb_map_paired_job is pinned to the oracle by
-test_fragment_distribution.py; here the device job must reproduce it byte for byte: records, both pools up to the used
-counts, status, pair routes and the distribution afterwards.  The CPU tests rehearse the driver's window cut and pool
-order with a host-side model."""
+ambiguous-pair buffer) on reads already in HBM.  Both jobs train through the same window step, so the training rule is
+checked against the oracle job (here and in test_fragment_distribution.py); here the device job must also reproduce the
+host job gb_map_paired_job byte for byte: records, both pools up to the used counts, status, pair routes and the
+distribution afterwards.  The CPU tests rehearse the driver's window cut and pool order with a host-side model."""
 import ctypes as C
 import os
 
@@ -147,8 +147,12 @@ def learn_params():
 
 
 def host_job(dev, reads, quals, f, p, window=0):
-    rbuf, qbuf, off = H.pack_reads(list(reads), None if quals is None else list(quals))
-    aln, maps, edits, status, route = dev.map_paired_job(rbuf, qbuf, off, f, p, training_window=window)
+    return host_job_on(dev, H.pack_reads(list(reads), None if quals is None else list(quals)), f, p, window)
+
+
+def host_job_on(dev, bufs, f, p, window=0):
+    """gb_map_paired_job on (reads, quals, read_off) in host memory."""
+    aln, maps, edits, status, route = dev.map_paired_job(*bufs, f, p, training_window=window)
     nm, ne = dev.last_used
     return aln, maps[:nm], edits[:ne], status, route
 
@@ -170,6 +174,8 @@ class DeviceReads:
                 qb[s:s + len(q)] = q
         self.n = len(reads)
         self.max_len = max((len(r) for r in reads), default=0)
+        # the same buffers in host memory, for the host job
+        self.host = (np.frombuffer(bytes(rb), np.uint8), None if quals is None else np.frombuffer(bytes(qb), np.uint8), np.array(off, np.uint64))
         self.reads = torch.frombuffer(rb, dtype=torch.uint8).cuda()
         self.quals = None if quals is None else torch.frombuffer(qb, dtype=torch.uint8).cuda()
         self.off = torch.tensor(off, dtype=torch.int64).cuda()
@@ -212,6 +218,16 @@ def fstate(f):
     return f.mean(), f.std_dev(), f.curr_sample_size(), f.is_finalized()
 
 
+def assert_oracle_job(got, f, index, reads, quals, max_n, freq):
+    """Routes, (mean, stdev, sample size) and records of the oracle job on the same reads."""
+    orc = H.oracle_map_paired_job(index, reads, quals, learn_params(), max_n, freq, 0.95, threads=8)
+    assert (got[4] == orc[4]).all(), "pair routes differ from the oracle job"
+    assert (f.mean(), f.std_dev(), f.curr_sample_size()) == orc[5]
+    full = (got[0], np.concatenate([got[1], np.zeros(1, capi.mapping_dt)]), np.concatenate([got[2], np.zeros(1, np.uint32)]), got[3])
+    bad = H.compare_alignments(full, orc, len(got[0]))
+    assert not bad, f"{len(bad)} reads differ from the oracle job; first: {bad[0]}"
+
+
 def both_jobs(dev, reads, quals, max_n, freq, window, p=None, **kw):
     p = p or learn_params()
     fh, fd = capi.FragmentDistribution(max_n, freq, 0.95), capi.FragmentDistribution(max_n, freq, 0.95)
@@ -230,13 +246,7 @@ def test_equals_host_job(dev, graph, n_pairs, max_n, freq, window):
     got, want, fh, fd = both_jobs(dev, rs.reads, rs.quals, max_n, freq, window)
     assert_same(got, want)
     assert fstate(fd) == fstate(fh) and fd.is_finalized()
-    if n_pairs == 400:
-        # and once directly against the oracle job
-        orc = H.oracle_map_paired_job(index, rs.reads, rs.quals, learn_params(), max_n, freq, 0.95, threads=8)
-        assert (got[4] == orc[4]).all()
-        assert (fd.mean(), fd.std_dev(), fd.curr_sample_size()) == orc[5]
-        full = (got[0], np.concatenate([got[1], np.zeros(1, capi.mapping_dt)]), np.concatenate([got[2], np.zeros(1, np.uint32)]), got[3])
-        assert not H.compare_alignments(full, orc, rs.n)
+    assert_oracle_job(got, fd, index, rs.reads, rs.quals, max_n, freq)
 
 
 @pytest.mark.gpu
@@ -248,6 +258,8 @@ def test_window_independence(dev):
         rc, got, _ = device_job(dev, DeviceReads(rs.reads, rs.quals), f, learn_params(), window)
         assert rc == capi.GB_OK
         outs.append((got, fstate(f)))
+        fh = capi.FragmentDistribution(200, 50, 0.95)
+        outs.append((host_job(dev, rs.reads, rs.quals, fh, learn_params(), window), fstate(fh)))
     for got, st in outs[1:]:
         assert_same(got, outs[0][0])
         assert st == outs[0][1]
@@ -309,16 +321,19 @@ def test_input_ending_before_the_sample_fills_and_the_fallback_limit(dev):
 
 
 @pytest.mark.gpu
-def test_unreachable_mates_register_minus_one(dev):
+def test_unreachable_mates_register_minus_one(dev, graph):
     """Mate 2 replaced by a forward-strand read from elsewhere: both ends map uniquely at full score, but the flipped mate 2
-    lies on the other strand, so the distance is unreachable (-1), which is below max_fragment_length and is registered."""
-    g = synth.make_variant_graph(length=150000, n_snp=240, n_ins=30, n_del=30, n_haps=8, seed=12)
+    lies on the other strand, so the distance is unreachable (-1), which is below max_fragment_length and is registered.
+    Both jobs train through one window step, so the oracle job is what checks that rule here."""
+    g, index = graph
     rs = synth.simulate_pairs(g, 300, sub_rate=0.0, seed=17)
     other = synth.simulate_pairs(g, 300, sub_rate=0.0, seed=18)
     reads = [bytes(rs.reads[i]) if i % 2 == 0 or (i // 2) % 3 else bytes(other.reads[i - 1]) for i in range(rs.n)]
     got, want, fh, fd = both_jobs(dev, reads, list(rs.quals), 100, 100, 0)
     assert_same(got, want)
     assert fstate(fd) == fstate(fh) and fd.curr_sample_size() == 100
+    assert_oracle_job(want, fh, index, reads, list(rs.quals), 100, 100)
+    assert_oracle_job(got, fd, index, reads, list(rs.quals), 100, 100)
 
 
 @pytest.mark.gpu
@@ -391,15 +406,19 @@ def test_refusals_and_optional_arrays(dev):
 
 @pytest.mark.gpu
 def test_offsets_with_a_base_and_gaps(dev):
-    """Offsets that start after a prefix give the records of zero-based ones.  Bytes between reads belong to the read
-    before them (read r is [off[r], off[r + 1])), so reads with gaps are compared with the host job on those longer reads."""
+    """Offsets that start after a prefix give the records of zero-based ones, in both jobs (the host job uploads each
+    training window and rebases its offsets).  Bytes between reads belong to the read before them (read r is
+    [off[r], off[r + 1])), so reads with gaps are compared with the host job on those longer reads."""
     _, rs = _job_inputs(500, seed=8)
     outs = []
     for prefix in (0, 1000, 37):
         f = capi.FragmentDistribution(150, 50, 0.95)
-        rc, got, _ = device_job(dev, DeviceReads(rs.reads, rs.quals, prefix=prefix), f, learn_params(), 64)
+        dr = DeviceReads(rs.reads, rs.quals, prefix=prefix)
+        rc, got, _ = device_job(dev, dr, f, learn_params(), 64)
         assert rc == capi.GB_OK
         outs.append((got, fstate(f)))
+        fh = capi.FragmentDistribution(150, 50, 0.95)
+        outs.append((host_job_on(dev, dr.host, fh, learn_params(), 64), fstate(fh)))
     for got, st in outs[1:]:
         assert_same(got, outs[0][0])
         assert st == outs[0][1]
@@ -413,6 +432,9 @@ def test_offsets_with_a_base_and_gaps(dev):
     assert rc == capi.GB_OK
     assert_same(got, want)
     assert fstate(fd) == fstate(fh)
+    fb = capi.FragmentDistribution(150, 50, 0.95)
+    assert_same(host_job_on(dev, dr.host, fb, learn_params(), 64), want)
+    assert fstate(fb) == fstate(fh)
     # max_read_len below the longest read is refused
     rc, _, _ = device_job(dev, dr, capi.FragmentDistribution(150, 50, 0.95), learn_params(), 64, max_read_len=150)
     assert rc == capi.GB_ERR_ARG

@@ -220,12 +220,9 @@ extern "C" int gb_device_create(const gb_flat_index* ix, int device_ordinal, gb_
             if ((rc = d->slots.upload(ix->slots, ix->n_slots, d->stream))) return rc;
             if ((rc = d->site_dist.upload(ix->site_dist, ix->site_dist_len ? ix->site_dist_len : 1, d->stream, ix->site_dist_len))) return rc;
             GB_CUDA(cudaStreamSynchronize(d->stream));
-            d->h_slots.assign(ix->slots, ix->slots + ix->n_slots);
-            d->h_site_dist.assign(ix->site_dist, ix->site_dist + ix->site_dist_len);
         }
         d->ix.slots = ix->n_slots ? d->slots.ptr : nullptr; d->ix.n_slots = (uint32_t)ix->n_slots; d->ix.site_dist = ix->n_slots ? d->site_dist.ptr : nullptr;
         d->h_node_len.resize(ix->n_nodes);
-        d->h_dist.assign(ix->dist, ix->dist + ix->n_nodes / 2);
         for (uint32_t v = 0; v < ix->n_nodes; v++) d->h_node_len[v] = ix->nodes[v].len;
         // c_in = x_in + offset and c_out = x_out - (length - offset) are int32 in the seeding kernels.  A derived payload
         // always fits (x_in + length is at most the graph's sequence, below 2^31 by the 32-bit seq_off); a hand-made one may not.

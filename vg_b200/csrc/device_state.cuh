@@ -124,13 +124,22 @@ int map_device(gb_device* d, const gb_map_params* hp, uint32_t n_reads, const ui
 // refuses (GB_ERR_CAPACITY) once they are at 1024x the per-read averages.
 int grow_pools_for_rerun(gb_device* d);
 
+// Read 1 of a pair, L1 bases long, takes map_paired's single-end fallback when the fragment limit (mean +
+// paired_distance_stdevs * stdev) is below its distance limit (minimizer_mapper.cpp:1469-1471).
+__host__ __device__ inline bool single_end_fallback(int64_t fragment_limit, int64_t distance_limit, int64_t L1) {
+    const int64_t read_limit = L1 + 50;
+    return fragment_limit < (distance_limit > read_limit ? distance_limit : read_limit);
+}
+// The refusal of a paired batch in which only some pairs take the fallback.
+inline constexpr char MIXED_FALLBACK_REFUSAL[] = "fragment distance limit below the read distance limit for some pairs only (mixed single-end "
+                                                 "fallback, minimizer_mapper.cpp:1471, is not supported in one batch)";
+
 } // namespace gb
 
 struct gb_device {
     int device = 0;
     int n_sms = 0;
     std::vector<uint32_t> h_node_len;      // host copy of the node lengths (workspace sizing of the DP seams)
-    std::vector<gb_dist_payload> h_dist;   // host copy of the distance payload (fragment-length training)
     bool chain_coords_fit = true;          // every used node's chain coordinates fit the mapping kernels' int32 c_in / c_out
     // first-pass seeding table sizes (minimizers, clusters per read); GIRAFFE_B200_SEED_TABLES="Mc,Cc" overrides
     uint32_t seed_mc = 64, seed_cc = 16, seed_ns = 64;
@@ -147,7 +156,6 @@ struct gb_device {
     gb::DevBuf<gb_hit> hits;
     gb::DevBuf<uint32_t> slot_order;
     gb::DevBuf<gb_slot_rec> slots; gb::DevBuf<uint16_t> site_dist;
-    std::vector<gb_slot_rec> h_slots; std::vector<uint16_t> h_site_dist;      // host copies (fragment-length training)
     gb::DevBuf<gb::QEntry> ws_queue;
     gb::DevBuf<gb::ArenaNode> ws_arena;
     gb::DevBuf<uint32_t> p_post;                     // items extend_kernel hands to extend_finish_kernel
@@ -217,7 +225,7 @@ struct gb_device {
     gb::DevBuf<uint8_t> bgzf_ws;           // gb_bgzf_compress_device: member slots, token slots, member sizes and offsets
     gb::DevBuf<uint8_t> inflate_ws;        // gb_bgzf_decompress_device: the member list and the walk's summary
     gb::DevBuf<uint8_t> fastq_ws;          // gb_fastq_parse_device: line ends, per-read lengths and offsets, scan temporaries
-    // gb_map_paired_job_device: one sub-batch's records, its gathered reads, the per-pair training arrays, the buffered pairs
+    // the paired jobs: one sub-batch's records, its gathered or uploaded reads, the per-pair training arrays, the buffered pairs
     struct PairedJobWs {
         gb::DevBuf<gb_alignment> aln;
         gb::DevBuf<uint8_t> status, reads, quals, scan_tmp;

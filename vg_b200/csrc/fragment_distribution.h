@@ -1,6 +1,5 @@
 // fragment_distribution.h — FragmentLengthDistribution (mapper.hpp:83-139, mapper.cpp:5231-5333), the state behind the
-// opaque gb_fragment_distribution handle.  Shared by the host paired job (paired_job.cu, which also defines estimate())
-// and the device-resident one (paired_job_device.cu).
+// opaque gb_fragment_distribution handle.  The paired jobs and estimate() are in paired_job.cu.
 #pragma once
 #include "giraffe_b200.h"
 

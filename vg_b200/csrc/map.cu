@@ -576,17 +576,15 @@ static int map_batch_host(gb_device* d, const gb_map_params* hp, bool paired,
         // (get_distance_limit of read 1); a batch where only some pairs fail it is refused.
         const int64_t fragment_limit = (int64_t)(hp->fragment_mean + hp->paired_distance_stdevs * hp->fragment_stdev);
         uint32_t fallback = 0;
-        for (uint32_t p = 0; p < n_reads / 2; p++) {
-            const int64_t L1 = (int64_t)(read_off[2 * (size_t)p + 1] - read_off[2 * (size_t)p]);
-            fallback += fragment_limit < std::max<int64_t>(hp->distance_limit, L1 + 50);
-        }
+        for (uint32_t p = 0; p < n_reads / 2; p++)
+            fallback += gb::single_end_fallback(fragment_limit, hp->distance_limit, (int64_t)(read_off[2 * (size_t)p + 1] - read_off[2 * (size_t)p]));
         if (fallback == n_reads / 2) {
             const int rcs = map_batch_host(d, hp, false, n_reads, reads, quals, read_off, aln, mappings, mapping_pool_cap, edits, edit_pool_cap,
                                            status, n_mappings_used, n_edits_used);
             if (rcs == GB_OK) for (size_t r = 0; r < (size_t)n_reads * K; r++) if (!(aln[r].flags & GB_ALN_ABSENT)) aln[r].flags |= GB_ALN_PAIRED;
             return rcs;
         }
-        if (fallback != 0) { g_last_error = "fragment distance limit below the read distance limit for some pairs only (mixed single-end fallback, minimizer_mapper.cpp:1471, is not supported in one batch)"; return GB_ERR_ARG; }
+        if (fallback != 0) { g_last_error = gb::MIXED_FALLBACK_REFUSAL; return GB_ERR_ARG; }
     }
     GB_CUDA(cudaSetDevice(d->device));
     const uint32_t chunk = d->map_chunk;
